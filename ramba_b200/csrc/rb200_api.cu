@@ -9,6 +9,8 @@
 
 #include "rb200_launch.h"
 #include "rb200_handlers.h"
+#include "rb200_stream.h"
+#include "rb200_tile.h"
 
 namespace rb200 {
 __global__ void fill_u64_kernel(u64* p, long long n, u64 bits) {
@@ -59,14 +61,15 @@ static int dtype_size(int dt) {
   }
 }
 
-static int g_sm_count = 0;
+static std::atomic<int> g_sm_count{0};
 static int sm_count() {
-  if (g_sm_count > 0) return g_sm_count;
+  const int cached = g_sm_count.load();
+  if (cached > 0) return cached;
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return -1;
   int n = 0;
   if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return -1;
-  g_sm_count = n;
+  g_sm_count.store(n);
   return n;
 }
 
@@ -142,18 +145,21 @@ static void assign_handlers(KParams& P, const rb200_fused_op* op, int set) {
   }
 }
 
-extern "C" {
+// ---- debugging aids (A/B measurements, bisecting a parity failure), read once: each takes a kernel family, the TMA
+// loader or the row tiling out of the selection, in the launch and in rb200_describe_plan alike
+struct KillSwitches {
+  bool no_tile, no_stream, no_mapred, no_terms, no_tma, no_row_mode;
+};
+static const KillSwitches& kill_switches() {
+  static const KillSwitches k = {getenv("RB200_NO_TILE_KERNEL") != nullptr,   getenv("RB200_NO_STREAM_KERNEL") != nullptr,
+                                 getenv("RB200_NO_MAPRED_KERNEL") != nullptr, getenv("RB200_NO_TERMS_KERNEL") != nullptr,
+                                 getenv("RB200_NO_TMA") != nullptr,           getenv("RB200_NO_ROW_MODE") != nullptr};
+  return k;
+}
 
-const char* rb200_last_error(void) { return g_last_error.c_str(); }
-int rb200_abi_version(void) { return RB200_ABI_VERSION; }
-int64_t rb200_launch_count(void) { return (int64_t)g_launches.load(); }
-void rb200_reset_launch_count(void) { g_launches.store(0); }
-int rb200_device_sm_count(void) { return sm_count(); }
-int64_t rb200_red_scratch_bytes(void) { return (int64_t)(256 + 8 * RB200_MAX_REDS * kRedScratchPartials); }
-
-
-
-int rb200_run_deferred_ops(const rb200_fused_op* op, void* stream_v) {
+// Every rejection of an op list, before any device query.  0: valid (*empty: an empty range, nothing to run), else the
+// status of fail().
+static int validate(const rb200_fused_op* op, bool* empty) {
   if (!op) return fail("null fused op");
   if (op->abi_version != RB200_ABI_VERSION) return fail("ABI version mismatch between caller and libramba_b200");
   if (op->ndim < 1 || op->ndim > RB200_MAX_DIMS) return fail("ndim out of range");
@@ -162,29 +168,15 @@ int rb200_run_deferred_ops(const rb200_fused_op* op, void* stream_v) {
   if (op->n_insns < 0 || op->n_insns > RB200_MAX_INSNS) return fail("too many instructions");
   if (op->n_regs < 0 || op->n_regs > RB200_MAX_REGS) return fail("too many spill registers");
   if (op->n_reds < 0 || op->n_reds > RB200_MAX_REDS) return fail("too many reductions");
-  cudaStream_t stream = (cudaStream_t)stream_v;
-
-  // the 1-D kernel owns 8 elements per thread, the N-d and axis kernels 4
-  const int V = (op->ndim == 1 && op->n_axis_red_dims == 0) ? kV1 : kV;
-  const long long TILE = (long long)kThreads * V;
-  KParams P;
-  memset(&P, 0, sizeof(P));
-  P.ndim = op->ndim;
-  P.n_insns = op->n_insns;
-  P.n_views = op->n_views;
-  P.n_regs = op->n_regs;
-  P.n_reds = op->n_reds;
   long long total = 1;
   for (int d = 0; d < op->ndim; ++d) {
     if (op->itershape[d] < 0) return fail("negative itershape");
     if (op->ndim > 1 && op->itershape[d] >= (1ll << 31)) return fail("N-d iteration dims must be < 2^31");
-    P.shape[d] = op->itershape[d];
-    P.gstart[d] = op->global_start[d];
     total *= op->itershape[d];
   }
-  if (total == 0 || op->n_insns == 0) return 0;  // empty range: nothing to do
+  *empty = total == 0 || op->n_insns == 0;
+  if (*empty) return 0;
 
-  bool view_read[RB200_MAX_VIEWS] = {false}, view_masked[RB200_MAX_VIEWS] = {false};
   for (int i = 0; i < op->n_insns; ++i) {
     const rb200_insn& I = op->insns[i];
     if (I.op >= RB200_NUM_OPS) return fail("bad opcode");
@@ -201,10 +193,7 @@ int rb200_run_deferred_ops(const rb200_fused_op* op, void* stream_v) {
         case RB200_K_NONE:
         case RB200_K_ACC: break;
         case RB200_K_REG: if (idxs[q] >= op->n_regs) return fail("register index out of range"); break;
-        case RB200_K_VIEW:
-          if (idxs[q] >= op->n_views) return fail("view index out of range");
-          view_read[idxs[q]] = true;
-          break;
+        case RB200_K_VIEW: if (idxs[q] >= op->n_views) return fail("view index out of range"); break;
         case RB200_K_SCAL: if (idxs[q] >= op->n_scalars) return fail("scalar index out of range"); break;
         case RB200_K_IOTA: if (idxs[q] >= op->ndim) return fail("iota dim out of range"); break;
         default: return fail("bad operand kind");
@@ -213,58 +202,203 @@ int rb200_run_deferred_ops(const rb200_fused_op* op, void* stream_v) {
     if (I.st_reg != RB200_NOSTORE && I.st_reg >= op->n_regs) return fail("st_reg out of range");
     if (I.st_view != RB200_NOSTORE && I.st_view >= op->n_views) return fail("st_view out of range");
     if (I.mask_reg != RB200_NOSTORE && I.mask_reg >= op->n_regs) return fail("mask_reg out of range");
-    if (I.st_view != RB200_NOSTORE && I.mask_reg != RB200_NOSTORE) view_masked[I.st_view] = true;
     if (I.op == RB200_OP_SINCOS && I.st2 >= op->n_regs) return fail("sincos st2 out of range");
     if (I.op == RB200_OP_RED && I.b_idx >= op->n_reds) return fail("reduction slot out of range");
+  }
+  for (int i = 0; i < op->n_views; ++i) {
+    if (dtype_size(op->views[i].dtype) == 0) return fail("bad view dtype");
+    if (!op->views[i].base) return fail("null view base pointer");
+  }
+  if (op->n_axis_red_dims != 0) {
+    // axis mode: the first n_axis_red_dims dims are the reduced ones (host permutes)
+    if (op->n_axis_red_dims >= op->ndim) return fail("axis reduction needs at least one kept dim");
+    if (op->n_reds < 1) return fail("axis reduction without reduction slots");
+    if (!op->red_scratch) return fail("axis reduction needs a partial buffer");
+  } else if (op->n_reds > 0) {
+    if (!op->red_scratch) return fail("global reduction needs red_scratch");
+    for (int s = 0; s < op->n_reds; ++s) {
+      if (!op->reds[s].out) return fail("null reduction output");
+      if (dtype_size(op->reds[s].out_dtype) == 0) return fail("bad reduction output dtype");
+      if (op->reds[s].ctype != RB200_T_F64 && op->reds[s].ctype != RB200_T_I64) return fail("reduction class must be F64 or I64");
+    }
+  }
+  return 0;
+}
+
+enum PlanForm { FORM_NONE, FORM_TILE, FORM_STREAM, FORM_AXIS_AS_1D, FORM_AXIS_REDUCE, FORM_ELEMENTWISE };
+
+// Which kernel runs one op list, and everything its launch needs.  One per call: nothing is shared between calls.
+struct Plan {
+  PlanForm form;
+  TilePlan tile;      // FORM_TILE
+  StreamPlan stream;  // FORM_STREAM
+  KParams k;          // the general interpreter forms
+  long long blocks;   // the general interpreter forms: grid and dynamic shared memory
+  size_t smem;
+  // axis reductions: the kernel writes splits [0, n_written) of n_split; launch() fills the rest with the identity
+  int n_split, n_written;
+  long long kept;
+  u64* partials;
+  u64 identity;
+};
+
+// axis-as-1-D form: [R reduced rows][C kept elements], every view contiguous over the box or broadcast over the rows,
+// C a multiple of the 1-D tile, one reduction slot, no index operands: the staged 1-D kernel with V column accumulators
+// per thread (rb200_elementwise_ax1d.cu).  false: not of this form, or its shared memory does not fit.
+static bool plan_axis_as_1d(const rb200_fused_op* op, int sms, const bool* view_read, size_t reg_bytes, Plan& pl) {
+  const KParams& P = pl.k;
+  const long long TILE1 = (long long)kThreads * kV1;
+  const long long red_len = P.red_len, kept = P.total;
+  bool ok = (op->ndim == 2 && P.red_ndim == 1 && op->n_reds == 1 && kept % TILE1 == 0 && kept / TILE1 <= (long long)sms * 2 && red_len >= 2);
+  for (int i = 0; i < op->n_insns && ok; ++i) {
+    const rb200_insn& I = op->insns[i];
+    if (I.a_kind == RB200_K_IOTA || I.b_kind == RB200_K_IOTA || I.c_kind == RB200_K_IOTA) ok = false;
+    if (I.st_view != RB200_NOSTORE) ok = false;  // stage 1 of an axis reduction only reads
+    if (I.op == RB200_OP_SINCOS && I.c_kind == RB200_K_VIEW) ok = false;  // (the parked-half store is a write too)
+  }
+  for (int i = 0; i < op->n_views && ok; ++i) {
+    const rb200_view& v = op->views[i];
+    if (!view_read[i]) continue;
+    if (v.stride[1] != 1 || !(v.stride[0] == kept || v.stride[0] == 0)) ok = false;
+  }
+  if (!ok) return false;
+  KParams Q = P;
+  const int V1 = kV1;
+  Q.ndim = 1;
+  Q.total = red_len * kept;
+  Q.n_tiles = Q.total / TILE1;
+  Q.shape[0] = Q.total;
+  Q.gstart[0] = 0;
+  Q.wide = 1;
+  const int n_chunks = (int)(kept / TILE1);
+  long long cap1 = (long long)sms * 2;
+  int n_split_eff = (int)(cap1 / n_chunks);
+  if (n_split_eff > P.n_split) n_split_eff = P.n_split;
+  if ((long long)n_split_eff > red_len) n_split_eff = (int)red_len;
+  if (n_split_eff < 1) n_split_eff = 1;
+  Q.n_split_chunks = n_chunks;
+  Q.n_split = n_split_eff;
+  Q.red_len = kept;  // in this mode: elements per row (partials are [split][kept])
+  Q.n_pf = 0;
+  for (int i = 0; i < op->n_views; ++i) {
+    KView& k = Q.views[i];
+    const rb200_view& v = op->views[i];
+    k.stride[0] = 1;
+    k.pf_slot = -1;
+    if (!view_read[i]) continue;
+    const int dt = v.dtype;
+    const bool wide_ok = (dt == RB200_F64 || dt == RB200_F32 || dt == RB200_I64 || dt == RB200_I32);
+    if (v.stride[0] == 0) {
+      k.pf_slot = -2;  // periodic: broadcast over the rows
+    } else if (wide_ok && Q.n_pf < kMaxPf && reg_bytes + (size_t)(Q.n_pf + 1) * 2 * V1 * kThreads * 8 <= 108 * 1024) {
+      k.pf_slot = Q.n_pf;
+      Q.pf_view[Q.n_pf] = i;
+      Q.n_pf++;
+    }
+  }
+  // hoist periodic views into extra spill registers when every use agrees on the compute class
+  for (int i = 0; i < op->n_views && Q.n_hoist < kMaxPf; ++i) {
+    if (Q.views[i].pf_slot != -2 || Q.n_regs >= RB200_MAX_REGS) continue;
+    int cls = -1;
+    bool same = true;
+    for (int q = 0; q < Q.n_insns; ++q) {
+      const rb200_insn& I = Q.insns[q];
+      const int use_cls = (I.op == RB200_OP_CVT) ? (int)(I.imm & 0xff) : (int)I.ctype;
+      const bool uses = (I.a_kind == RB200_K_VIEW && I.a_idx == i) || (I.b_kind == RB200_K_VIEW && I.b_idx == i && I.op != RB200_OP_RED) ||
+                        (I.c_kind == RB200_K_VIEW && I.c_idx == i && I.op != RB200_OP_SINCOS);
+      if (!uses) continue;
+      if (I.op == RB200_OP_POWI && I.b_kind == RB200_K_VIEW && I.b_idx == i) same = false;  // integer exponent operand
+      if (cls < 0) cls = use_cls;
+      else if (cls != use_cls) same = false;
+    }
+    if (cls < 0 || !same) continue;
+    const int r = Q.n_regs++;
+    Q.hoist_view[Q.n_hoist] = i;
+    Q.hoist_reg[Q.n_hoist] = r;
+    Q.hoist_cls[Q.n_hoist] = cls;
+    Q.n_hoist++;
+    for (int q = 0; q < Q.n_insns; ++q) {
+      rb200_insn& I = Q.insns[q];
+      if (I.a_kind == RB200_K_VIEW && I.a_idx == i) { I.a_kind = RB200_K_REG; I.a_idx = (uint8_t)r; }
+      if (I.b_kind == RB200_K_VIEW && I.b_idx == i && I.op != RB200_OP_RED) { I.b_kind = RB200_K_REG; I.b_idx = (uint8_t)r; }
+      if (I.c_kind == RB200_K_VIEW && I.c_idx == i && I.op != RB200_OP_SINCOS) { I.c_kind = RB200_K_REG; I.c_idx = (uint8_t)r; }
+    }
+  }
+  const size_t reg_bytes1 = (size_t)(Q.n_regs + 1) * V1 * kThreads * 8;
+  Q.bulk = Q.n_pf > 0 ? 1 : 0;
+  for (int j = 0; j < Q.n_pf; ++j)
+    if ((((uintptr_t)op->views[Q.pf_view[j]].base) & 15u) != 0) Q.bulk = 0;
+  Q.n_stages = 2;
+  const size_t pf_bytes1 = (size_t)Q.n_pf * Q.n_stages * V1 * kThreads * 8;
+  if (reg_bytes1 + pf_bytes1 > 200 * 1024) return false;  // does not fit: the general axis kernel runs it
+  assign_handlers(Q, op, 1);
+  pl.k = Q;
+  pl.form = FORM_AXIS_AS_1D;
+  pl.blocks = (long long)n_split_eff * n_chunks;
+  pl.smem = reg_bytes1 + pf_bytes1;
+  pl.n_written = n_split_eff;
+  return true;
+}
+
+// The kernel choice for a valid, non-empty op list on a device with `sms` multiprocessors.  The only decisions left to
+// the launch are the driver's: encoding a TMA tensor map (the cooperative loader when that fails).
+static void make_plan(const rb200_fused_op* op, int sms, Plan& pl) {
+  const KillSwitches& ks = kill_switches();
+  pl.form = FORM_NONE;
+  pl.n_split = pl.n_written = 0;
+  // ---- specialised kernels first: float-arithmetic op lists over 2-D / 3-D boxes (shifted-view stencils with the
+  // halo tile staged in shared memory by TMA, and N-d elementwise maps) run on the lean machine of rb200_tile.cu
+  if (!ks.no_tile && plan_stencil_tile(op, sms, !ks.no_terms, !ks.no_tma, pl.tile)) {
+    pl.form = FORM_TILE;
+    return;
+  }
+  // float-arithmetic op lists over a contiguous 1-D space (incl. global reductions): the streaming kernel
+  if (op->ndim == 1 && op->n_axis_red_dims == 0 && !ks.no_stream &&
+      plan_stream(op, sms, kRedScratchPartials, 0, !ks.no_terms, !ks.no_mapred, pl.stream)) {
+    pl.form = FORM_STREAM;
+    return;
+  }
+
+  // ---- the general interpreter
+  // the 1-D kernel owns 8 elements per thread, the N-d and axis kernels 4
+  const int V = (op->ndim == 1 && op->n_axis_red_dims == 0) ? kV1 : kV;
+  const long long TILE = (long long)kThreads * V;
+  KParams& P = pl.k;
+  memset(&P, 0, sizeof(P));
+  P.ndim = op->ndim;
+  P.n_insns = op->n_insns;
+  P.n_views = op->n_views;
+  P.n_regs = op->n_regs;
+  P.n_reds = op->n_reds;
+  long long total = 1;
+  for (int d = 0; d < op->ndim; ++d) {
+    P.shape[d] = op->itershape[d];
+    P.gstart[d] = op->global_start[d];
+    total *= op->itershape[d];
+  }
+  bool view_read[RB200_MAX_VIEWS] = {false}, view_masked[RB200_MAX_VIEWS] = {false};
+  for (int i = 0; i < op->n_insns; ++i) {
+    const rb200_insn& I = op->insns[i];
+    const uint8_t kinds[3] = {I.a_kind, I.b_kind, I.c_kind};
+    const uint8_t idxs[3] = {I.a_idx, I.b_idx, I.c_idx};
+    for (int q = 0; q < 3; ++q)
+      if (kinds[q] == RB200_K_VIEW && !(I.op == RB200_OP_RED && q == 1) && !(I.op == RB200_OP_SINCOS && q == 2)) view_read[idxs[q]] = true;
+    if (I.st_view != RB200_NOSTORE && I.mask_reg != RB200_NOSTORE) view_masked[I.st_view] = true;
     P.insns[i] = I;
   }
   for (int i = 0; i < op->n_scalars; ++i) P.scalars[i] = op->scalars[i];
-
   for (int i = 0; i < op->n_views; ++i) {
     const rb200_view& v = op->views[i];
-    const int es = dtype_size(v.dtype);
-    if (es == 0) return fail("bad view dtype");
-    if (!v.base) return fail("null view base pointer");
     KView& k = P.views[i];
     k.base = (char*)v.base;
     k.dtype = v.dtype;
     k.pf_slot = -1;
     for (int d = 0; d < op->ndim; ++d) k.stride[d] = v.stride[d];
   }
-  // the op list is valid; from here on a device is needed (there is no CPU path)
-  const int sms = sm_count();
-  if (sms <= 0) return fail("no usable CUDA device (libramba_b200 has no CPU path)");
-  cudaError_t e;
   const size_t reg_bytes = (size_t)(op->n_regs + 1) * V * kThreads * 8;  // + the scratch column of the out-of-line stores
 
-  // ---- specialised kernels first: float-arithmetic op lists over 2-D / 3-D boxes (shifted-view stencils with the
-  // halo tile staged in shared memory by TMA, and N-d elementwise maps) run on the lean machine of rb200_tile.cu
-  {
-    std::string terr;
-    const int r = launch_stencil_tile(op, sms, stream, &terr);
-    if (r == 0) {
-      g_launches.fetch_add(1);
-      return 0;
-    }
-    if (r == 2) return fail(terr);
-  }
-  // float-arithmetic op lists over a contiguous 1-D space (incl. global reductions): the streaming kernel
-  if (op->ndim == 1 && op->n_axis_red_dims == 0) {
-    std::string terr;
-    const int r = launch_stream_1d(op, sms, kRedScratchPartials, stream, &terr);
-    if (r == 0) {
-      g_launches.fetch_add(1);
-      return 0;
-    }
-    if (r == 2) return fail(terr);
-  }
-
   if (op->n_axis_red_dims != 0) {
-    // axis mode: the first n_axis_red_dims dims are the reduced ones (host permutes)
     const int nred = op->n_axis_red_dims;
-    if (nred >= op->ndim) return fail("axis reduction needs at least one kept dim");
-    if (op->n_reds < 1) return fail("axis reduction without reduction slots");
-    if (!op->red_scratch) return fail("axis reduction needs a partial buffer");
     P.red_ndim = nred;
     long long red_len = 1, kept = 1;
     for (int d = 0; d < nred; ++d) red_len *= P.shape[d];
@@ -282,136 +416,25 @@ int rb200_run_deferred_ops(const rb200_fused_op* op, void* stream_v) {
       P.reds[s].op = op->reds[s].op;
       P.reds[s].ctype = op->reds[s].ctype;
     }
+    pl.n_split = n_split;
+    pl.kept = kept;
+    pl.partials = (u64*)op->red_scratch;
+    pl.identity = host_red_identity_bits(op->reds[0].op, op->reds[0].ctype);
     // ---- column form on the streaming kernel of the lean machine (float arithmetic op lists)
-    {
-      std::string terr;
-      int eff = 0;
-      const int r = launch_stream_columns(op, sms, n_split, stream, &eff, &terr);
-      if (r == 2) return fail(terr);
-      if (r == 0) {
-        g_launches.fetch_add(1);
-        if (eff < n_split) {
-          const long long n_fill = (long long)(n_split - eff) * kept;
-          fill_u64_kernel<<<(unsigned)((n_fill + 255) / 256 > 1184 ? 1184 : (n_fill + 255) / 256), 256, 0, stream>>>(
-              (u64*)op->red_scratch + (long long)eff * kept, n_fill, host_red_identity_bits(op->reds[0].op, op->reds[0].ctype));
-          e = cudaGetLastError();
-          if (e != cudaSuccess) return fail_cuda("fill_u64_kernel launch", e);
-          g_launches.fetch_add(1);
-        }
-        return 0;
-      }
+    if (!ks.no_stream && plan_stream(op, sms, kRedScratchPartials, n_split, !ks.no_terms, !ks.no_mapred, pl.stream)) {
+      pl.form = FORM_STREAM;
+      pl.n_written = pl.stream.eff;
+      return;
     }
-    // ---- axis-as-1-D fast path: [R reduced rows][C kept elements], every view contiguous over the box
-    // or broadcast over the rows, C a multiple of the 1-D tile, one reduction slot, no index operands:
-    // run the staged 1-D kernel with V column accumulators per thread (rb200_elementwise_ax1d.cu)
-    {
-      const long long TILE1 = (long long)kThreads * kV1;
-      bool ok = (op->ndim == 2 && nred == 1 && op->n_reds == 1 && kept % TILE1 == 0 && kept / TILE1 <= (long long)sms * 2 && red_len >= 2);
-      for (int i = 0; i < op->n_insns && ok; ++i) {
-        const rb200_insn& I = op->insns[i];
-        if (I.a_kind == RB200_K_IOTA || I.b_kind == RB200_K_IOTA || I.c_kind == RB200_K_IOTA) ok = false;
-        if (I.st_view != RB200_NOSTORE) ok = false;  // stage 1 of an axis reduction only reads
-        if (I.op == RB200_OP_SINCOS && I.c_kind == RB200_K_VIEW) ok = false;  // (the parked-half store is a write too)
-      }
-      for (int i = 0; i < op->n_views && ok; ++i) {
-        const rb200_view& v = op->views[i];
-        if (!view_read[i]) continue;
-        if (v.stride[1] != 1 || !(v.stride[0] == kept || v.stride[0] == 0)) ok = false;
-      }
-      if (ok) {
-        KParams Q = P;
-        const int V1 = kV1;
-        Q.ndim = 1;
-        Q.total = red_len * kept;
-        Q.n_tiles = Q.total / TILE1;
-        Q.shape[0] = Q.total;
-        Q.gstart[0] = 0;
-        Q.wide = 1;
-        const int n_chunks = (int)(kept / TILE1);
-        long long cap1 = (long long)sms * 2;
-        int n_split_eff = (int)(cap1 / n_chunks);
-        if (n_split_eff > n_split) n_split_eff = n_split;
-        if ((long long)n_split_eff > red_len) n_split_eff = (int)red_len;
-        if (n_split_eff < 1) n_split_eff = 1;
-        Q.n_split_chunks = n_chunks;
-        Q.n_split = n_split_eff;
-        Q.red_len = kept;  // in this mode: elements per row (partials are [split][kept])
-        Q.n_pf = 0;
-        size_t pf_bytes1 = 0;
-        for (int i = 0; i < op->n_views; ++i) {
-          KView& k = Q.views[i];
-          const rb200_view& v = op->views[i];
-          k.stride[0] = 1;
-          k.pf_slot = -1;
-          if (!view_read[i]) continue;
-          const int dt = v.dtype;
-          const bool wide_ok = (dt == RB200_F64 || dt == RB200_F32 || dt == RB200_I64 || dt == RB200_I32);
-          if (v.stride[0] == 0) {
-            k.pf_slot = -2;  // periodic: broadcast over the rows
-          } else if (wide_ok && Q.n_pf < kMaxPf && reg_bytes + (size_t)(Q.n_pf + 1) * 2 * V1 * kThreads * 8 <= 108 * 1024) {
-            k.pf_slot = Q.n_pf;
-            Q.pf_view[Q.n_pf] = i;
-            Q.n_pf++;
-          }
-        }
-        // hoist periodic views into extra spill registers when every use agrees on the compute class
-        for (int i = 0; i < op->n_views && Q.n_hoist < kMaxPf; ++i) {
-          if (Q.views[i].pf_slot != -2 || Q.n_regs >= RB200_MAX_REGS) continue;
-          int cls = -1;
-          bool same = true;
-          for (int q = 0; q < Q.n_insns; ++q) {
-            const rb200_insn& I = Q.insns[q];
-            const int use_cls = (I.op == RB200_OP_CVT) ? (int)(I.imm & 0xff) : (int)I.ctype;
-            const bool uses = (I.a_kind == RB200_K_VIEW && I.a_idx == i) || (I.b_kind == RB200_K_VIEW && I.b_idx == i && I.op != RB200_OP_RED) ||
-                              (I.c_kind == RB200_K_VIEW && I.c_idx == i && I.op != RB200_OP_SINCOS);
-            if (!uses) continue;
-            if (I.op == RB200_OP_POWI && I.b_kind == RB200_K_VIEW && I.b_idx == i) same = false;  // integer exponent operand
-            if (cls < 0) cls = use_cls;
-            else if (cls != use_cls) same = false;
-          }
-          if (cls < 0 || !same) continue;
-          const int r = Q.n_regs++;
-          Q.hoist_view[Q.n_hoist] = i;
-          Q.hoist_reg[Q.n_hoist] = r;
-          Q.hoist_cls[Q.n_hoist] = cls;
-          Q.n_hoist++;
-          for (int q = 0; q < Q.n_insns; ++q) {
-            rb200_insn& I = Q.insns[q];
-            if (I.a_kind == RB200_K_VIEW && I.a_idx == i) { I.a_kind = RB200_K_REG; I.a_idx = (uint8_t)r; }
-            if (I.b_kind == RB200_K_VIEW && I.b_idx == i && I.op != RB200_OP_RED) { I.b_kind = RB200_K_REG; I.b_idx = (uint8_t)r; }
-            if (I.c_kind == RB200_K_VIEW && I.c_idx == i && I.op != RB200_OP_SINCOS) { I.c_kind = RB200_K_REG; I.c_idx = (uint8_t)r; }
-          }
-        }
-        const size_t reg_bytes1 = (size_t)(Q.n_regs + 1) * V1 * kThreads * 8;
-        Q.bulk = Q.n_pf > 0 ? 1 : 0;
-        for (int j = 0; j < Q.n_pf; ++j)
-          if ((((uintptr_t)op->views[Q.pf_view[j]].base) & 15u) != 0) Q.bulk = 0;
-        Q.n_stages = 2;
-        pf_bytes1 = (size_t)Q.n_pf * Q.n_stages * V1 * kThreads * 8;
-        if (reg_bytes1 + pf_bytes1 > 200 * 1024) goto general_axis;  // does not fit: use the general kernel
-        assign_handlers(Q, op, 1);
-        e = launch_vm_elementwise_ax1d(Q, (unsigned)(n_split_eff * n_chunks), reg_bytes1 + pf_bytes1, stream);
-        if (e != cudaSuccess) return fail_cuda("vm_elementwise_kernel (axis-as-1-D) launch", e);
-        g_launches.fetch_add(1);
-        if (n_split_eff < n_split) {
-          const long long n_fill = (long long)(n_split - n_split_eff) * kept;
-          fill_u64_kernel<<<(unsigned)((n_fill + 255) / 256 > 1184 ? 1184 : (n_fill + 255) / 256), 256, 0, stream>>>(
-              (u64*)op->red_scratch + (long long)n_split_eff * kept, n_fill, host_red_identity_bits(op->reds[0].op, op->reds[0].ctype));
-          e = cudaGetLastError();
-          if (e != cudaSuccess) return fail_cuda("fill_u64_kernel launch", e);
-          g_launches.fetch_add(1);
-        }
-        return 0;
-      }
-    }
-  general_axis:
+    if (plan_axis_as_1d(op, sms, view_read, reg_bytes, pl)) return;
     long long blocks = P.n_tiles;
     long long cap = (long long)sms * 4;
     if (blocks > cap) blocks = cap;
-    e = launch_vm_axis_reduce(P, (unsigned)blocks, reg_bytes, stream);
-    if (e != cudaSuccess) return fail_cuda("vm_axis_reduce_kernel launch", e);
-    g_launches.fetch_add(1);
-    return 0;
+    pl.form = FORM_AXIS_REDUCE;
+    pl.blocks = blocks;
+    pl.smem = reg_bytes;
+    pl.n_written = n_split;
+    return;
   }
 
   P.total = total;
@@ -422,8 +445,7 @@ int rb200_run_deferred_ops(const rb200_fused_op* op, void* stream_v) {
     // tile instead of once per element (no per-element divisions); used when rows fill their tiles well
     const long long inner = op->itershape[op->ndim - 1];
     const long long chunks = (inner + TILE - 1) / TILE;
-    static const bool row_mode_off = getenv("RB200_NO_ROW_MODE") != nullptr;  // debugging aid: always take the flat mode
-    if (!row_mode_off && inner * 5 >= chunks * TILE * 4 && chunks < (1ll << 30)) {
+    if (!ks.no_row_mode && inner * 5 >= chunks * TILE * 4 && chunks < (1ll << 30)) {
       P.row_chunks = (int)chunks;
       P.n_tiles = (total / inner) * chunks;
     }
@@ -473,13 +495,9 @@ int rb200_run_deferred_ops(const rb200_fused_op* op, void* stream_v) {
   const size_t smem = reg_bytes + pf_bytes + ocls_bytes;
   assign_handlers(P, op, op->ndim == 1 ? 1 : 2);
   if (op->n_reds > 0) {
-    if (!op->red_scratch) return fail("global reduction needs red_scratch");
     P.red_counter = (unsigned int*)op->red_scratch;
     P.red_partials = (u64*)((char*)op->red_scratch + 256);
     for (int s = 0; s < op->n_reds; ++s) {
-      if (!op->reds[s].out) return fail("null reduction output");
-      if (dtype_size(op->reds[s].out_dtype) == 0) return fail("bad reduction output dtype");
-      if (op->reds[s].ctype != RB200_T_F64 && op->reds[s].ctype != RB200_T_I64) return fail("reduction class must be F64 or I64");
       P.reds[s].op = op->reds[s].op;
       P.reds[s].ctype = op->reds[s].ctype;
       P.reds[s].out = op->reds[s].out;
@@ -498,37 +516,109 @@ int rb200_run_deferred_ops(const rb200_fused_op* op, void* stream_v) {
   long long cap = (long long)sms * per_sm;
   if (op->n_reds > 0 && cap > kRedScratchPartials) cap = kRedScratchPartials;
   if (blocks > cap) blocks = cap;
-  switch (op->ndim) {
-    case 1: e = launch_vm_elementwise_nd1(P, (unsigned)blocks, smem, stream); break;
-    case 2: e = launch_vm_elementwise_nd2(P, (unsigned)blocks, smem, stream); break;
-    case 3: e = launch_vm_elementwise_nd3(P, (unsigned)blocks, smem, stream); break;
-    default: e = launch_vm_elementwise_nd5(P, (unsigned)blocks, smem, stream); break;
+  pl.form = FORM_ELEMENTWISE;
+  pl.blocks = blocks;
+  pl.smem = smem;
+}
+
+// what a failed launch of the plan's kernel was, for rb200_last_error
+static std::string launch_failure(const Plan& pl) {
+  const KParams& P = pl.k;
+  char buf[256];
+  switch (pl.form) {
+    case FORM_TILE: {
+      const TilePlan& T = pl.tile;
+      snprintf(buf, sizeof(buf), "stencil_tile_kernel launch (blocks=%lld smem=%zu group=%d tma=%d)", T.blocks, T.smem, T.P.has_group, T.P.use_tma);
+    } break;
+    case FORM_STREAM: {
+      const StreamPlan& T = pl.stream;
+      snprintf(buf, sizeof(buf), "stream kernel%s launch (blocks=%lld smem=%zu staged=%d depth=%d terms=%d)", T.P.mode == 1 ? " (columns)" : "", T.blocks,
+               T.smem, T.P.n_staged, T.P.depth, T.P.n_terms);
+    } break;
+    case FORM_AXIS_AS_1D: return "vm_elementwise_kernel (axis-as-1-D) launch";
+    case FORM_AXIS_REDUCE: return "vm_axis_reduce_kernel launch";
+    default:
+      snprintf(buf, sizeof(buf), "vm_elementwise_kernel launch (ndim=%d blocks=%lld smem=%zu n_regs=%d n_pf=%d n_insns=%d)", P.ndim, pl.blocks, pl.smem,
+               P.n_regs, P.n_pf, P.n_insns);
   }
-  if (e != cudaSuccess) {
-    char buf[256];
-    snprintf(buf, sizeof(buf), "vm_elementwise_kernel launch (ndim=%d blocks=%lld smem=%zu n_regs=%d n_pf=%d n_insns=%d)", op->ndim, blocks, smem,
-             op->n_regs, P.n_pf, op->n_insns);
-    return fail_cuda(buf, e);
+  return buf;
+}
+
+// Launches the plan's kernel and, for an axis reduction whose kernel writes fewer splits than requested, fills the rest
+// with the identity.  No choices are made here.
+static int launch(Plan& pl, cudaStream_t stream) {
+  const KParams& P = pl.k;
+  const unsigned blocks = (unsigned)pl.blocks;
+  cudaError_t e = cudaSuccess;
+  switch (pl.form) {
+    case FORM_NONE: return 0;
+    case FORM_TILE: e = launch_stencil_tile(pl.tile, stream); break;
+    case FORM_STREAM: e = launch_stream(pl.stream, stream); break;
+    case FORM_AXIS_AS_1D: e = launch_vm_elementwise_ax1d(P, blocks, pl.smem, stream); break;
+    case FORM_AXIS_REDUCE: e = launch_vm_axis_reduce(P, blocks, pl.smem, stream); break;
+    case FORM_ELEMENTWISE:
+      switch (P.ndim) {
+        case 1: e = launch_vm_elementwise_nd1(P, blocks, pl.smem, stream); break;
+        case 2: e = launch_vm_elementwise_nd2(P, blocks, pl.smem, stream); break;
+        case 3: e = launch_vm_elementwise_nd3(P, blocks, pl.smem, stream); break;
+        default: e = launch_vm_elementwise_nd5(P, blocks, pl.smem, stream); break;
+      }
+      break;
   }
+  if (e != cudaSuccess) return fail_cuda(launch_failure(pl).c_str(), e);
   g_launches.fetch_add(1);
+  if (pl.n_written < pl.n_split) {
+    const long long n_fill = (long long)(pl.n_split - pl.n_written) * pl.kept;
+    fill_u64_kernel<<<(unsigned)((n_fill + 255) / 256 > 1184 ? 1184 : (n_fill + 255) / 256), 256, 0, stream>>>(pl.partials + (long long)pl.n_written * pl.kept,
+                                                                                                               n_fill, pl.identity);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return fail_cuda("fill_u64_kernel launch", e);
+    g_launches.fetch_add(1);
+  }
   return 0;
 }
 
+static std::string describe(const rb200_fused_op* op, const Plan& pl) {
+  if (pl.form == FORM_TILE) return describe_stencil_tile(pl.tile);
+  if (pl.form == FORM_STREAM) return describe_stream(pl.stream);
+  if (pl.form == FORM_NONE) return "kernel=none";
+  const char* form = pl.form == FORM_ELEMENTWISE ? "elementwise" : pl.form == FORM_AXIS_AS_1D ? "axis_as_1d" : "axis_reduce";
+  const char* tiling = pl.form != FORM_ELEMENTWISE || op->ndim == 1 ? "" : pl.k.row_chunks > 0 ? " tiling=row" : " tiling=flat";
+  char buf[200];
+  snprintf(buf, sizeof(buf), "kernel=general_interpreter form=%s ndim=%d insns=%d views=%d%s ctas=%lld smem=%zu", form, op->ndim, op->n_insns, op->n_views,
+           tiling, pl.blocks, pl.smem);
+  return buf;
+}
+
+extern "C" {
+
+const char* rb200_last_error(void) { return g_last_error.c_str(); }
+int rb200_abi_version(void) { return RB200_ABI_VERSION; }
+int64_t rb200_launch_count(void) { return (int64_t)g_launches.load(); }
+void rb200_reset_launch_count(void) { g_launches.store(0); }
+int rb200_device_sm_count(void) { return sm_count(); }
+int64_t rb200_red_scratch_bytes(void) { return (int64_t)(256 + 8 * RB200_MAX_REDS * kRedScratchPartials); }
+
+int rb200_run_deferred_ops(const rb200_fused_op* op, void* stream_v) {
+  bool empty = false;
+  if (const int rc = validate(op, &empty)) return rc;
+  if (empty) return 0;  // empty range: nothing to do
+  // the op list is valid; from here on a device is needed (there is no CPU path)
+  const int sms = sm_count();
+  if (sms <= 0) return fail("no usable CUDA device (libramba_b200 has no CPU path)");
+  Plan pl;
+  make_plan(op, sms, pl);
+  return launch(pl, (cudaStream_t)stream_v);
+}
+
 int rb200_describe_plan(const rb200_fused_op* op, char* out, int64_t cap) {
-  if (!op || !out || cap < 2) return fail("describe_plan: null argument");
-  if (op->abi_version != RB200_ABI_VERSION) return fail("ABI version mismatch between caller and libramba_b200");
-  if (op->ndim < 1 || op->ndim > RB200_MAX_DIMS || op->n_views < 0 || op->n_views > RB200_MAX_VIEWS || op->n_insns < 0 ||
-      op->n_insns > RB200_MAX_INSNS || op->n_scalars < 0 || op->n_scalars > RB200_MAX_SCALARS || op->n_reds < 0 || op->n_reds > RB200_MAX_REDS)
-    return fail("describe_plan: malformed fused op");
-  const int sms = 132;  // H100 SXM; the plan does not depend on a device being present
-  std::string d;
-  if (!(op->n_axis_red_dims == 0 && describe_stencil_tile(op, sms, &d)) && !describe_stream(op, sms, &d)) {
-    char buf[160];
-    snprintf(buf, sizeof(buf), "kernel=general_interpreter form=%s ndim=%d insns=%d views=%d", op->n_axis_red_dims ? "axis_reduce" : "elementwise", op->ndim,
-             op->n_insns, op->n_views);
-    d = buf;
-  }
-  snprintf(out, (size_t)cap, "%s", d.c_str());
+  if (!out || cap < 2) return fail("describe_plan: null argument");
+  bool empty = false;
+  if (const int rc = validate(op, &empty)) return rc;
+  Plan pl;
+  pl.form = FORM_NONE;
+  if (!empty) make_plan(op, 132, pl);  // H100 SXM; the plan does not depend on a device being present
+  snprintf(out, (size_t)cap, "%s", describe(op, pl).c_str());
   return 0;
 }
 

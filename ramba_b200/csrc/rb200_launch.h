@@ -1,6 +1,4 @@
 #pragma once
-#include <string>
-
 #include "rb200_vm.cuh"
 
 namespace rb200 {
@@ -13,13 +11,6 @@ cudaError_t launch_vm_elementwise_nd3(const KParams& P, unsigned blocks, size_t 
 cudaError_t launch_vm_elementwise_nd5(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream);
 cudaError_t launch_vm_elementwise_ax1d(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream);
 cudaError_t launch_vm_axis_reduce(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream);
-// specialised kernels tried before the general interpreter.  Return 0: launched, 1: the op list is not of their form
-// (fall through), 2: error (*err set)
-int launch_stencil_tile(const rb200_fused_op* op, int sms, cudaStream_t stream, std::string* err);
-int launch_stream_1d(const rb200_fused_op* op, int sms, int max_red_blocks, cudaStream_t stream, std::string* err);
-int launch_stream_columns(const rb200_fused_op* op, int sms, int n_split, cudaStream_t stream, int* n_split_eff_out, std::string* err);
-bool describe_stencil_tile(const rb200_fused_op* op, int sms, std::string* out);
-bool describe_stream(const rb200_fused_op* op, int sms, std::string* out);
 long long scan_scratch_bytes(long long n_outer, long long len, long long n_inner);
 cudaError_t launch_scan(const void* src, void* dst, int dtype, long long n_outer, long long len, long long n_inner, int op, const void* carry, void* totals,
                         void* scratch, int sms, cudaStream_t stream, bool* supported);

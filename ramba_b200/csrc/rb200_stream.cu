@@ -28,52 +28,9 @@
 #include "rb200_lean_plan.h"
 #include "rb200_terms.h"
 #include "rb200_mapred.h"
+#include "rb200_stream.h"
 
 namespace rb200 {
-
-constexpr int kStreamMaxStaged = 4;
-
-
-constexpr int kStreamTile = LV * kThreads;  // 2048
-
-struct StreamStaged {
-  const char* base;
-  int es;        // element size (4 / 8)
-  int dview;     // the same view in the direct table (ragged last tile)
-  unsigned off;  // byte offset inside a stage
-  int pad;
-};
-
-struct StreamHoist {
-  int direct, reg, is_f32_class;
-};
-
-struct StreamParams {
-  int mode;
-  long long total, n_tiles;                  // mode 0
-  long long R, C, rows_per_split;            // mode 1: box [R][C]
-  int n_chunks, n_split;
-  int n_staged, depth;
-  unsigned stage_bytes;
-  StreamStaged staged[kStreamMaxStaged];
-  int n_direct;
-  LDirect direct[RB200_MAX_VIEWS];           // s1: row stride (mode 1), s2: element / column stride
-  int n_hoist;
-  StreamHoist hoist[kStreamMaxStaged];
-  int n_insns, n_regs;
-  LInsn insns[RB200_MAX_INSNS];
-  u64 scal[RB200_MAX_SCALARS];
-  int n_reds;
-  KRed reds[RB200_MAX_REDS];
-  u64* red_partials;
-  unsigned int* red_counter;
-  // term form (n_terms > 0, stream_terms_kernel): tile = tv * 256 elements; steps [0, n32) in float32, the rest in float64
-  int tv, n_terms, n32;
-  int n_thoist;                      // column mode: row-broadcast operands copied once per CTA into shared memory
-  int thoist_direct[kStreamMaxStaged];
-  TermStep terms[kMaxTerms];
-};
-constexpr int X_HOIST = 3;  // TermStep.xkind of the streaming kernel: element of a hoisted (row-broadcast) operand
 
 struct StreamCtx {
   const StreamParams& P;
@@ -839,7 +796,7 @@ static void stream_layout(StreamParams& P) {
 static size_t stream_smem(StreamParams& P) {
   const size_t tile = (size_t)P.tv * kThreads;
   const size_t regs = P.n_terms > 0 ? (size_t)P.n_thoist * tile * 8 : (size_t)(P.n_regs + P.n_hoist) * LV * kThreads * 8;
-  const size_t budget = (P.n_terms > 0 && P.tv == 8) ? 70 * 1024 : 100 * 1024;  // (term kernel, 8 per thread: 3 CTAs per SM)
+  const size_t budget = P.n_terms > 0 ? 70 * 1024 : 100 * 1024;  // (term kernel: 3 CTAs per SM)
   if (regs + 1024 > budget) return 0;
   int depth = 0;
   if (P.n_staged > 0) {
@@ -851,40 +808,30 @@ static size_t stream_smem(StreamParams& P) {
   return (size_t)depth * P.stage_bytes + regs + (size_t)(depth > 0 ? depth : 1) * 8 + 16;
 }
 
-struct StreamPlan {
-  StreamParams P;
-  size_t smem;
-  long long blocks;
-  int eff;  // column mode: splits actually written
-  bool use_mr;  // the map + reduce kernels of rb200_mapred.cu run this op list
-  MrParams mr;
-};
-
-// 0: planned, 1: not of this kernel's form
-static int stream_plan(const rb200_fused_op* op, int sms, int max_red_blocks, int n_split, StreamPlan& T) {
+bool plan_stream(const rb200_fused_op* op, int sms, int max_red_blocks, int n_split, bool use_terms, bool use_mapred, StreamPlan& T) {
   StreamParams& P = T.P;
   memset(&T, 0, sizeof(T));
   const bool column = op->n_axis_red_dims != 0;
   if (!column) {
-    if (op->ndim != 1) return 1;
-    if (!lean_eligible(op, true)) return 1;
+    if (op->ndim != 1) return false;
+    if (!lean_eligible(op, true)) return false;
     for (int s = 0; s < op->n_reds; ++s) {
-      if (op->reds[s].ctype != RB200_T_F64) return 1;
-      if (op->reds[s].out_dtype != RB200_F64 && op->reds[s].out_dtype != RB200_F32) return 1;
+      if (op->reds[s].ctype != RB200_T_F64) return false;
+      if (op->reds[s].out_dtype != RB200_F64 && op->reds[s].out_dtype != RB200_F32) return false;
     }
     P.mode = 0;
     P.total = op->itershape[0];
   } else {
-    if (op->ndim != 2 || op->n_axis_red_dims != 1 || op->n_reds != 1) return 1;
-    if (!lean_eligible(op, true)) return 1;
-    if (op->reds[0].ctype != RB200_T_F64) return 1;
+    if (op->ndim != 2 || op->n_axis_red_dims != 1 || op->n_reds != 1) return false;
+    if (!lean_eligible(op, true)) return false;
+    if (op->reds[0].ctype != RB200_T_F64) return false;
     const long long R = op->itershape[0], C = op->itershape[1];
-    if (C % (LV * kThreads) != 0 || R < 2) return 1;
+    if (C % (LV * kThreads) != 0 || R < 2) return false;
     for (int i = 0; i < op->n_insns; ++i)
-      if (op->insns[i].st_view != RB200_NOSTORE) return 1;
+      if (op->insns[i].st_view != RB200_NOSTORE) return false;
     for (int v = 0; v < op->n_views; ++v) {
       const rb200_view& vw = op->views[v];
-      if (vw.stride[1] != 1 || !(vw.stride[0] == C || vw.stride[0] == 0)) return 1;
+      if (vw.stride[1] != 1 || !(vw.stride[0] == C || vw.stride[0] == 0)) return false;
     }
     P.mode = 1;
     P.R = R;
@@ -894,7 +841,6 @@ static int stream_plan(const rb200_fused_op* op, int sms, int max_red_blocks, in
   P.tv = LV;
   stream_translate(op, P, column, P.C);
   // ---- the term form first
-  static const bool no_terms = getenv("RB200_NO_TERMS_KERNEL") != nullptr;  // debugging aid
   TermBuild tb;
   tb.n_regs = P.n_regs;
   tb.direct = P.direct;
@@ -902,12 +848,8 @@ static int stream_plan(const rb200_fused_op* op, int sms, int max_red_blocks, in
   tb.staged_fill = [](void*, int, int, TermStep*) -> bool { return true; };
   tb.ctx = nullptr;
   int out_view = -1;
-  bool all_f32 = true;
-  for (int v = 0; v < op->n_views; ++v)
-    if (op->views[v].dtype != RB200_F32) all_f32 = false;
-  if (!no_terms && build_terms(tb, P.insns, P.n_insns, P.terms, kMaxTerms, &P.n_terms, &P.n32, &out_view)) {
+  if (use_terms && build_terms(tb, P.insns, P.n_insns, P.terms, kMaxTerms, &P.n_terms, &P.n32, &out_view)) {
     // ---- one contiguous source, scalar map, one reduction: the map + reduce kernels (no staging, no interpretation)
-    static const bool no_mr = getenv("RB200_NO_MAPRED_KERNEL") != nullptr;  // debugging aid
     auto src_of = [](void* ctx, const TermStep& t) -> MrSource {
       const StreamParams* Q = (const StreamParams*)ctx;
       MrSource r = {nullptr, 0, false};
@@ -921,7 +863,7 @@ static int stream_plan(const rb200_fused_op* op, int sms, int max_red_blocks, in
       r.row_broadcast = Q->mode == 1 && d->s1 == 0;
       return r;
     };
-    if (!no_mr && op->n_reds == 1 && mapred_try(P.mode, P.terms, P.n_terms, P.n32, P.scal, src_of, &P, &T.mr) == 0) {
+    if (use_mapred && op->n_reds == 1 && mapred_try(P.mode, P.terms, P.n_terms, P.n32, P.scal, src_of, &P, &T.mr) == 0) {
       MrParams& M = T.mr;
       const int vec = M.src_f32 ? 4 : 2;
       bool ok = true;
@@ -960,11 +902,9 @@ static int stream_plan(const rb200_fused_op* op, int sms, int max_red_blocks, in
       if (ok) {
         T.use_mr = true;
         T.smem = 0;
-        return 0;
+        return true;
       }
     }
-    static const bool tv8 = getenv("RB200_STREAM_TV16") != nullptr;  // debugging aid: 16 elements per thread
-    if (all_f32 && tv8 && (!column || P.C % (16 * kThreads) == 0)) P.tv = 16;  // (16 per thread spills: 8 per thread at 3 CTAs per SM is the default)
     stream_layout(P);
     if (column) {
       // row-broadcast direct operands: one copy per CTA in shared memory
@@ -989,7 +929,7 @@ static int stream_plan(const rb200_fused_op* op, int sms, int max_red_blocks, in
     if (column) stream_hoist_lean(P);
   }
   T.smem = stream_smem(P);
-  if (T.smem == 0) return 1;
+  if (T.smem == 0) return false;
   const long long tile = (long long)P.tv * kThreads;
   P.n_reds = op->n_reds;
   for (int s = 0; s < op->n_reds; ++s) {
@@ -1005,14 +945,14 @@ static int stream_plan(const rb200_fused_op* op, int sms, int max_red_blocks, in
       P.red_partials = (u64*)((char*)op->red_scratch + 256);
     }
     long long blocks = P.n_tiles;
-    long long cap = (long long)sms * ((P.n_terms > 0 && P.tv == 8 && T.smem <= 72 * 1024) ? RB200_STREAM_MINB8 : 2);
+    long long cap = (long long)sms * ((P.n_terms > 0 && T.smem <= 72 * 1024) ? RB200_STREAM_MINB8 : 2);
     if (op->n_reds > 0 && cap > max_red_blocks) cap = max_red_blocks;
     if (blocks > cap) blocks = cap;
     T.blocks = blocks;
   } else {
     P.n_chunks = (int)(P.C / tile);
-    const int per_sm = (P.n_terms > 0 && P.tv == 8 && T.smem <= 72 * 1024) ? RB200_STREAM_MINB8 : 2;
-    if (P.n_chunks > sms * per_sm) return 1;
+    const int per_sm = (P.n_terms > 0 && T.smem <= 72 * 1024) ? RB200_STREAM_MINB8 : 2;
+    if (P.n_chunks > sms * per_sm) return false;
     int eff = (int)(((long long)sms * per_sm) / P.n_chunks);
     if (n_split > 0 && eff > n_split) eff = n_split;
     if ((long long)eff > P.R) eff = (int)P.R;
@@ -1023,86 +963,36 @@ static int stream_plan(const rb200_fused_op* op, int sms, int max_red_blocks, in
     T.eff = eff;
     T.blocks = (long long)eff * P.n_chunks;
   }
-  return 0;
+  return true;
 }
 
-static cudaError_t stream_launch(const StreamParams& P, unsigned blocks, size_t smem, cudaStream_t stream) {
-  static bool attr = false;
-  if (!attr) {
-    cudaFuncSetAttribute(stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 101 * 1024);
-    cudaFuncSetAttribute(stream_terms_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 101 * 1024);
-    cudaFuncSetAttribute(stream_terms_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 101 * 1024);
-    attr = true;
-  }
-  if (P.n_terms > 0) {
-    if (P.tv == 16) stream_terms_kernel<16><<<blocks, kThreads, smem, stream>>>(P);
-    else stream_terms_kernel<8><<<blocks, kThreads, smem, stream>>>(P);
-  } else {
-    stream_kernel<<<blocks, kThreads, smem, stream>>>(P);
-  }
-  return cudaGetLastError();
-}
-
-// one line for rb200_describe_plan; false: not this kernel's form
-bool describe_stream(const rb200_fused_op* op, int sms, std::string* out) {
-  static StreamPlan T;
-  if (stream_plan(op, sms, 4096, op->axis_nsplit, T) != 0) return false;
+std::string describe_stream(const StreamPlan& T) {
   const StreamParams& P = T.P;
   char buf[320];
   if (T.use_mr) {
     snprintf(buf, sizeof(buf), "kernel=mapred mode=%s source=%s ops=%d(f32:%d) broadcast_operand=%d reduction=%d loads=128bit ctas=%lld", P.mode == 0 ? "global" : "columns",
              T.mr.src_f32 ? "f32" : "f64", T.mr.n32 + T.mr.n64, T.mr.n32, T.mr.vsrc ? 1 : 0, T.mr.redop, T.blocks);
-    *out = buf;
-    return true;
+    return buf;
   }
   snprintf(buf, sizeof(buf),
            "kernel=%s mode=%s staged_views=%d ring_depth=%d stage_bytes=%u direct_views=%d hoisted=%d lean_insns=%d terms=%d(f32:%d) tile=%d reds=%d "
            "ctas=%lld smem=%zu",
            P.n_terms > 0 ? "stream_terms" : "stream", P.mode == 0 ? "elementwise" : "columns", P.n_staged, P.depth, P.stage_bytes, P.n_direct,
-           P.n_terms > 0 ? P.n_thoist : P.n_hoist, P.n_insns, P.n_terms, P.n32, P.tv * kThreads, op->n_reds, T.blocks, T.smem);
-  *out = buf;
-  return true;
+           P.n_terms > 0 ? P.n_thoist : P.n_hoist, P.n_insns, P.n_terms, P.n32, P.tv * kThreads, P.n_reds, T.blocks, T.smem);
+  return buf;
 }
 
-// mode 0.  0: launched, 1: not of this form, 2: error
-int launch_stream_1d(const rb200_fused_op* op, int sms, int max_red_blocks, cudaStream_t stream, std::string* err) {
-  static const bool disabled = getenv("RB200_NO_STREAM_KERNEL") != nullptr;  // debugging aid
-  if (disabled) return 1;
-  if (op->ndim != 1 || op->n_axis_red_dims != 0) return 1;
-  for (int s = 0; s < op->n_reds; ++s)
-    if (!op->reds[s].out) return 1;
-  if (op->n_reds > 0 && !op->red_scratch) return 1;
-  static StreamPlan T;  // (large; launches are issued from one thread per process)
-  if (stream_plan(op, sms, max_red_blocks, 0, T) != 0) return 1;
-  const cudaError_t e = T.use_mr ? mapred_launch(T.mr, (unsigned)T.blocks, stream) : stream_launch(T.P, (unsigned)T.blocks, T.smem, stream);
-  if (e != cudaSuccess) {
-    char buf[200];
-    snprintf(buf, sizeof(buf), "stream kernel launch (blocks=%lld smem=%zu staged=%d depth=%d terms=%d): %s", T.blocks, T.smem, T.P.n_staged, T.P.depth,
-             T.P.n_terms, cudaGetErrorString(e));
-    *err = buf;
-    return 2;
-  }
-  return 0;
-}
-
-// mode 1: axis reduction over the rows of a [R][C] box into partials[n_split_eff][C].  On success *n_split_eff_out is
-// the number of splits written (the caller fills the remaining ones with the identity).
-int launch_stream_columns(const rb200_fused_op* op, int sms, int n_split, cudaStream_t stream, int* n_split_eff_out, std::string* err) {
-  static const bool disabled = getenv("RB200_NO_STREAM_KERNEL") != nullptr;
-  if (disabled) return 1;
-  if (op->ndim != 2 || op->n_axis_red_dims != 1 || op->n_reds != 1 || !op->red_scratch) return 1;
-  static StreamPlan T;
-  if (stream_plan(op, sms, 4096, n_split, T) != 0) return 1;
-  const cudaError_t e = T.use_mr ? mapred_launch(T.mr, (unsigned)T.blocks, stream) : stream_launch(T.P, (unsigned)T.blocks, T.smem, stream);
-  if (e != cudaSuccess) {
-    char buf[200];
-    snprintf(buf, sizeof(buf), "stream kernel (columns) launch (blocks=%lld smem=%zu staged=%d depth=%d terms=%d): %s", T.blocks, T.smem, T.P.n_staged,
-             T.P.depth, T.P.n_terms, cudaGetErrorString(e));
-    *err = buf;
-    return 2;
-  }
-  *n_split_eff_out = T.eff;
-  return 0;
+cudaError_t launch_stream(const StreamPlan& T, cudaStream_t stream) {
+  if (T.use_mr) return mapred_launch(T.mr, (unsigned)T.blocks, stream);
+  static const bool attrs = []() {  // (set once, thread-safe)
+    cudaFuncSetAttribute(stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 101 * 1024);
+    cudaFuncSetAttribute(stream_terms_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 101 * 1024);
+    return true;
+  }();
+  (void)attrs;
+  if (T.P.n_terms > 0) stream_terms_kernel<8><<<(unsigned)T.blocks, kThreads, T.smem, stream>>>(T.P);
+  else stream_kernel<<<(unsigned)T.blocks, kThreads, T.smem, stream>>>(T.P);
+  return cudaGetLastError();
 }
 
 }  // namespace rb200

@@ -33,55 +33,9 @@
 #include "rb200_lean.cuh"
 #include "rb200_lean_plan.h"
 #include "rb200_terms.h"
+#include "rb200_tile.h"
 
 namespace rb200 {
-
-constexpr int kTileMaxStaged = RB200_MAX_VIEWS;
-constexpr int kTileMaxRing = 8;
-// tile geometry (compile-time, so that every shared-memory access of an operand is base + immediate): 128 columns x
-// 16 rows of outputs per plane, element k of a thread is 2 rows below element k-1; the staged box is 144 columns wide
-// (halo <= 16 columns in total) and 16 + halo rows high
-constexpr int kTileTX = 128, kTileLogTX = 7, kTileRY = kThreads / kTileTX, kTileTY = LV * kTileRY, kTilePX = 144;
-constexpr int kTileMaxChain = 64;
-constexpr int kTilePrefetch = 2;  // planes requested ahead of the one being computed (1 when the ring would not fit)
-
-struct TileStagedOp {
-  int dzl;           // plane of the ring relative to the oldest needed plane (0 .. hz)
-  unsigned off;      // byte offset inside a plane: ((dy + hy_lo) * PX + dx + hx_lo) * elem
-};
-
-constexpr int kTileMaxTerms = kMaxTerms;
-
-struct TileParams {
-  long long Z, Y, X;        // iteration extents (Z == 1 for 2-D ops)
-  int nxt, nyt, nzc;        // tiles along x, y; chunks along z
-  long long ZC;             // planes per work item
-  long long n_items;
-  // staged group
-  int has_group, use_tma, elem;
-  int hz_lo, hz, hy_lo, hy, hx_lo, hx;  // halos: lo part and total (lo + hi)
-  int PY, D, prefetch;                   // rows of the plane box (kTilePX columns), ring depth, planes requested ahead
-  unsigned plane_bytes;
-  const char* gcorner;                   // address of group element (z = -hz_lo, y = -hy_lo, x = -hx_lo)
-  long long gs0, gs1;                    // group strides (elements) of z and y; x stride is 1
-  const char* safe_lo;                   // [safe_lo, safe_hi): bytes the cooperative loader may touch
-  const char* safe_hi;
-  int tma_shift;                         // elements the tensor-map base was moved down to reach 16-byte alignment
-  int n_staged;
-  TileStagedOp staged[kTileMaxStaged];
-  int n_direct;
-  LDirect direct[RB200_MAX_VIEWS];
-  int n_insns, n_regs;
-  LInsn insns[RB200_MAX_INSNS];
-  u64 scal[RB200_MAX_SCALARS];
-  LChainStep chain[kTileMaxChain];
-  // term form (n_terms > 0): steps [0, n32) run in float32, steps [n32, n_terms) in float64
-  int n_terms, n32, out_view;
-  int fast_tail;  // the float64 phase is exactly one `acc (+|-) w*x` term over a staged operand
-  int tv;  // elements per thread per plane of this launch (8, or 16 for the term kernel on float32 tiles): tile rows = tv * 2
-  TermStep terms[kTileMaxTerms];
-  unsigned char term_run[kTileMaxTerms];  // > 0: this and the next term_run-1 terms are plain `acc (+|-)= staged x` of one sign
-};
 
 __device__ __forceinline__ void tma_load_3d(unsigned sdst, const CUtensorMap* tmap, int c0, int c1, int c2, unsigned mbar) {
   asm volatile(
@@ -589,14 +543,12 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 static EncodeTiledFn encode_tiled_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
+  static const EncodeTiledFn fn = []() -> EncodeTiledFn {  // (initialised once, thread-safe)
     void* p = nullptr;
     cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess) fn = (EncodeTiledFn)p;
-  }
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess) return (EncodeTiledFn)p;
+    return nullptr;
+  }();
   return fn;
 }
 
@@ -606,30 +558,17 @@ static long long floor_div(long long a, long long b) {  // b > 0
   return q;
 }
 
-
-struct TilePlan {
-  TileParams P;
-  size_t smem;
-  long long blocks;
-  // TMA descriptor inputs (valid when tma_ok): base moved down to 16-byte alignment, halo'd extents
-  bool tma_ok;
-  const char* tbase;
-  long long Xh, Yh, Zh;
-  int shift, es, nd;
-};
-
-// 0: planned, 1: not eligible (caller falls back to the general interpreter)
-static int plan_stencil_tile(const rb200_fused_op* op, int sms, TilePlan& T) {
-  if (op->ndim != 2 && op->ndim != 3) return 1;
-  if (op->n_reds != 0 || op->n_axis_red_dims != 0) return 1;
-  if (!lean_eligible(op, false)) return 1;
+bool plan_stencil_tile(const rb200_fused_op* op, int sms, bool use_terms, bool use_tma, TilePlan& T) {
+  if (op->ndim != 2 && op->ndim != 3) return false;
+  if (op->n_reds != 0 || op->n_axis_red_dims != 0) return false;
+  if (!lean_eligible(op, false)) return false;
   const int nd = op->ndim;
   TileParams& P = T.P;
   memset(&T, 0, sizeof(T));
   P.Z = nd == 3 ? op->itershape[0] : 1;
   P.Y = op->itershape[nd - 2];
   P.X = op->itershape[nd - 1];
-  if (P.X >= (1ll << 31) || P.Y >= (1ll << 31) || P.Z >= (1ll << 31)) return 1;
+  if (P.X >= (1ll << 31) || P.Y >= (1ll << 31) || P.Z >= (1ll << 31)) return false;
 
   // ---- which views are read / written
   bool rd[RB200_MAX_VIEWS] = {false}, wr[RB200_MAX_VIEWS] = {false};
@@ -737,8 +676,8 @@ static int plan_stencil_tile(const rb200_fused_op* op, int sms, TilePlan& T) {
 
   // ---- staged operands: plane of the ring and byte offset inside a plane (rows of kTilePX elements)
   if (P.has_group) {
-    if (kTileTX + P.hx > kTilePX) return 1;
-    if (P.hz > 3) return 1;
+    if (kTileTX + P.hx > kTilePX) return false;
+    if (P.hz > 3) return false;
     for (int j = 0; j < P.n_staged; ++j) {
       P.staged[j].dzl = (int)(mdz[j] + P.hz_lo);
       P.staged[j].off = (unsigned)(((mdy[j] + P.hy_lo) * kTilePX + (mdx[j] + P.hx_lo)) * es);
@@ -760,7 +699,6 @@ static int plan_stencil_tile(const rb200_fused_op* op, int sms, TilePlan& T) {
   P.n_insns = op->n_insns;
   P.n_regs = op->n_regs;
   lean_translate(op, view_kind, view_arg, store_arg, P.insns);
-  static const bool no_terms = getenv("RB200_NO_TERMS_KERNEL") != nullptr;  // debugging aid: always the general tile kernel
   P.tv = LV;
   TermBuild tb;
   tb.n_regs = P.n_regs;
@@ -776,7 +714,7 @@ static int plan_stencil_tile(const rb200_fused_op* op, int sms, TilePlan& T) {
   };
   tb.ctx = &P;
   P.elem = es;
-  if (no_terms || !build_terms(tb, P.insns, P.n_insns, P.terms, kTileMaxTerms, &P.n_terms, &P.n32, &P.out_view)) {
+  if (!use_terms || !build_terms(tb, P.insns, P.n_insns, P.terms, kTileMaxTerms, &P.n_terms, &P.n32, &P.out_view)) {
     P.n_terms = 0;
     int n_chain = 0;
     P.n_insns = lean_fuse_chains(P.insns, P.n_insns, P.chain, kTileMaxChain, &n_chain);
@@ -800,9 +738,6 @@ static int plan_stencil_tile(const rb200_fused_op* op, int sms, TilePlan& T) {
       const TermStep& t = P.terms[P.n32];
       P.fast_tail = t.kind == TK_ADD && t.xkind == X_STAGED && (t.flags & TF_W) != 0 ? 1 : 0;
     }
-    // float32 tiles: 16 elements per thread (tile of 32 rows) halve the per-term and per-plane fixed cost per element
-    static const bool tv8 = getenv("RB200_TERMS_TV16") != nullptr;  // debugging aid: 16 elements per thread, 2 CTAs per SM
-    if (es == 4 && tv8) P.tv = 16;  // (measured: 8 elements per thread at 3 CTAs per SM beat 16 at 2: 2.18 vs 2.39 ms on 1024^3)
   }
   for (int i = 0; i < op->n_scalars; ++i) P.scal[i] = op->scalars[i];
 
@@ -813,20 +748,19 @@ static int plan_stencil_tile(const rb200_fused_op* op, int sms, TilePlan& T) {
   const size_t other = (P.n_terms > 0 ? (size_t)2 * kTileMaxTerms * 4 : (size_t)P.n_regs * LV * kThreads * 8) + kTileMaxRing * 8 + 16;
   if (P.has_group) {
     P.PY = TYr + P.hy;
-    if (P.PY > 256) return 1;
+    if (P.PY > 256) return false;
     P.plane_bytes = (unsigned)(((size_t)kTilePX * P.PY * es + 127) / 128 * 128);
     // ring = planes in use (hz + 1) + planes in flight; two in flight when that still leaves room for two CTAs per SM
-    static const int pf_env = getenv("RB200_TILE_PREFETCH") ? atoi(getenv("RB200_TILE_PREFETCH")) : 0;  // debugging aid
-    P.prefetch = pf_env >= 1 && pf_env <= 4 ? pf_env : kTilePrefetch;
+    P.prefetch = kTilePrefetch;
     while (P.prefetch > 1 && (size_t)(P.hz + 1 + P.prefetch) * P.plane_bytes + other > 100 * 1024) --P.prefetch;
     P.D = P.hz + 1 + P.prefetch;
-    if (P.D > kTileMaxRing) return 1;
+    if (P.D > kTileMaxRing) return false;
   }
   const size_t smem = (size_t)P.D * P.plane_bytes + other;
-  if (smem > 100 * 1024) return 1;  // (two CTAs per SM)
+  if (smem > 100 * 1024) return false;  // (two CTAs per SM)
 
   // ---- work items: z chunks so that every CTA of the persistent grid gets several
-  const long long grid_cap = (long long)sms * ((P.n_terms > 0 && P.tv == 8 && es == 4 && smem <= (220 * 1024) / RB200_TERMS_MINB - 1024) ? RB200_TERMS_MINB : 2);
+  const long long grid_cap = (long long)sms * ((P.n_terms > 0 && es == 4 && smem <= (220 * 1024) / RB200_TERMS_MINB - 1024) ? RB200_TERMS_MINB : 2);
   const long long xy = (long long)P.nxt * P.nyt;
   long long want_chunks = (grid_cap * 6 + xy - 1) / xy;
   if (want_chunks < 1) want_chunks = 1;
@@ -855,15 +789,12 @@ static int plan_stencil_tile(const rb200_fused_op* op, int sms, TilePlan& T) {
     const char* ahi = (const char*)op->views[best_ref].alloc_hi;
     const bool aligned = (P.gs1 * es) % 16 == 0 && (nd == 2 || ((P.gs0 * es) % 16 == 0 && P.gs0 > 0)) && (corner % (unsigned)es) == 0;
     const bool inside = T.tbase >= alo && far_end <= ahi;
-    T.tma_ok = aligned && inside && T.Xh < (1ll << 31);
+    T.tma_ok = use_tma && aligned && inside && T.Xh < (1ll << 31);
   }
-  return 0;
+  return true;
 }
 
-// one line for rb200_describe_plan; false: not this kernel's form
-bool describe_stencil_tile(const rb200_fused_op* op, int sms, std::string* out) {
-  TilePlan T;
-  if (plan_stencil_tile(op, sms, T) != 0) return false;
+std::string describe_stencil_tile(const TilePlan& T) {
   const TileParams& P = T.P;
   int n_chain_insns = 0, n_chain_steps = 0;
   for (int i = 0; i < P.n_insns; ++i)
@@ -877,26 +808,17 @@ bool describe_stencil_tile(const rb200_fused_op* op, int sms, std::string* out) 
            "chains=%d chain_steps=%d terms=%d(f32:%d) tile=128x%d items=%lld planes_per_item=%lld ctas=%lld smem=%zu",
            P.n_terms > 0 ? "stencil_terms" : "stencil_tile", T.es, P.Z, P.Y, P.X, P.n_staged, P.hz_lo, P.hz - P.hz_lo, P.hy_lo, P.hy - P.hy_lo, P.hx_lo, P.hx - P.hx_lo, P.D,
            !P.has_group ? "none" : (T.tma_ok ? "tma" : "cp.async"), P.n_direct, P.n_insns, n_chain_insns, n_chain_steps, P.n_terms, P.n32, P.tv * kTileRY, P.n_items, P.ZC, T.blocks, T.smem);
-  *out = buf;
-  return true;
+  return buf;
 }
 
-// 0: launched, 1: not eligible (caller falls back to the general interpreter), 2: error (*err set)
-int launch_stencil_tile(const rb200_fused_op* op, int sms, cudaStream_t stream, std::string* err) {
-  static const bool disabled = getenv("RB200_NO_TILE_KERNEL") != nullptr;  // debugging aid
-  if (disabled) return 1;
-  static TilePlan T;  // (large; launches are issued from one thread per process)
-  if (plan_stencil_tile(op, sms, T) != 0) return 1;
+cudaError_t launch_stencil_tile(TilePlan& T, cudaStream_t stream) {
   TileParams& P = T.P;
   const int es = T.es, nd = T.nd;
-  const size_t smem = T.smem;
-  const long long blocks = T.blocks;
   CUtensorMap tmap;
   memset(&tmap, 0, sizeof(tmap));
   if (P.has_group && T.tma_ok) {
-    static const bool no_tma = getenv("RB200_NO_TMA") != nullptr;  // debugging aid: always the cooperative loader
     EncodeTiledFn enc = encode_tiled_fn();
-    if (!no_tma && enc) {
+    if (enc) {
       cuuint64_t gdim[3] = {(cuuint64_t)T.Xh, (cuuint64_t)T.Yh, (cuuint64_t)T.Zh};
       cuuint64_t gstr[2] = {(cuuint64_t)(P.gs1 * es), (cuuint64_t)((nd == 3 ? P.gs0 : P.gs1 * T.Yh) * es)};
       cuuint32_t box[3] = {(cuuint32_t)kTilePX, (cuuint32_t)P.PY, 1};
@@ -911,33 +833,23 @@ int launch_stencil_tile(const rb200_fused_op* op, int sms, cudaStream_t stream, 
     }
   }
 
-  cudaError_t e;
-  static bool attrs = false;
-  if (!attrs) {
+  static const bool attrs = []() {  // (set once, thread-safe)
     cudaFuncSetAttribute(stencil_tile_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
     cudaFuncSetAttribute(stencil_tile_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
     cudaFuncSetAttribute(stencil_terms_kernel<double, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
     cudaFuncSetAttribute(stencil_terms_kernel<float, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-    cudaFuncSetAttribute(stencil_terms_kernel<float, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-    attrs = true;
-  }
+    return true;
+  }();
+  (void)attrs;
+  const unsigned blocks = (unsigned)T.blocks;
   if (P.n_terms > 0) {
-    if (es == 8) stencil_terms_kernel<double, 8><<<(unsigned)blocks, kThreads, smem, stream>>>(P, tmap);
-    else if (P.tv == 16) stencil_terms_kernel<float, 16><<<(unsigned)blocks, kThreads, smem, stream>>>(P, tmap);
-    else stencil_terms_kernel<float, 8><<<(unsigned)blocks, kThreads, smem, stream>>>(P, tmap);
+    if (es == 8) stencil_terms_kernel<double, 8><<<blocks, kThreads, T.smem, stream>>>(P, tmap);
+    else stencil_terms_kernel<float, 8><<<blocks, kThreads, T.smem, stream>>>(P, tmap);
   } else {
-    if (es == 8) stencil_tile_kernel<double><<<(unsigned)blocks, kThreads, smem, stream>>>(P, tmap);
-    else stencil_tile_kernel<float><<<(unsigned)blocks, kThreads, smem, stream>>>(P, tmap);
+    if (es == 8) stencil_tile_kernel<double><<<blocks, kThreads, T.smem, stream>>>(P, tmap);
+    else stencil_tile_kernel<float><<<blocks, kThreads, T.smem, stream>>>(P, tmap);
   }
-  e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    char buf[256];
-    snprintf(buf, sizeof(buf), "stencil_tile_kernel launch (blocks=%lld smem=%zu group=%d tma=%d): %s", blocks, smem, P.has_group, P.use_tma,
-             cudaGetErrorString(e));
-    *err = buf;
-    return 2;
-  }
-  return 0;
+  return cudaGetLastError();
 }
 
 }  // namespace rb200

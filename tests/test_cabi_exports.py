@@ -91,9 +91,18 @@ def _one_insn_op():
     return f
 
 
+def _null_reduction_output(f):
+    """A global reduction whose reds[0].out is null."""
+    from ramba_b200 import _cabi
+
+    f.n_reds = 1
+    f.red_scratch = 0x2000
+    f.reds[0].op, f.reds[0].ctype, f.reds[0].out_dtype = _cabi.RED_ADD, _cabi.T_F64, _cabi.F64
+
+
 def test_malformed_op_lists_are_rejected_with_a_reason():
     """Error convention of the boundary (include/ramba_b200.h): nonzero status + thread-local message; the op
-    list is validated before any device work, so this needs no GPU."""
+    list is validated before any device work, so this needs no GPU.  rb200_describe_plan validates the same way."""
     import ctypes as C
 
     from ramba_b200 import _cabi
@@ -105,6 +114,13 @@ def test_malformed_op_lists_are_rejected_with_a_reason():
         mutate(f)
         rc = lib.rb200_run_deferred_ops(C.byref(f), None)
         return rc, lib.rb200_last_error().decode()
+
+    def describe(mutate):
+        f = _one_insn_op()
+        mutate(f)
+        buf = C.create_string_buffer(600)
+        rc = lib.rb200_describe_plan(C.byref(f), buf, 600)
+        return rc, (lib.rb200_last_error() if rc else buf.value).decode()
 
     cases = [
         (lambda f: setattr(f, "abi_version", 99), "ABI version"),
@@ -120,13 +136,16 @@ def test_malformed_op_lists_are_rejected_with_a_reason():
         (lambda f: setattr(f.insns[0], "mask_reg", 1), "mask_reg out of range"),
         (lambda f: setattr(f.views[0], "dtype", 55), "bad view dtype"),
         (lambda f: setattr(f.views[0], "base", 0), "null view base pointer"),
+        (_null_reduction_output, "null reduction output"),
     ]
     for mutate, reason in cases:
-        rc, msg = run(mutate)
-        assert rc != 0 and reason in msg, (reason, rc, msg)
+        for call in (run, describe):
+            rc, msg = call(mutate)
+            assert rc != 0 and reason in msg, (call.__name__, reason, rc, msg)
     # an empty iteration space is a successful no-op
     rc, _ = run(lambda f: f.itershape.__setitem__(0, 0))
     assert rc == 0
+    assert describe(lambda f: f.itershape.__setitem__(0, 0)) == (0, "kernel=none")
     with pytest.raises(_cabi.CabiError):
         bad = _one_insn_op()
         bad.insns[0].op = 200
