@@ -27,7 +27,7 @@ from . import common
 from . import shardview
 from .common import dprint, timer, add_time
 from .program import E, Iota, Lowering, ProgramError, ProgramLimit, TempVar, dtype_class, rb_dtype
-from .runtime import RT, torch_dtype
+from .runtime import RT, _VERIFY_PLAN_CACHE, fill_template, torch_dtype
 
 int64 = np.int64
 float64 = np.float64
@@ -1019,87 +1019,18 @@ def _ring_receivable(bd_dist, vd, exec_dist, w, W, shard):
     return True
 
 
-_plan_cache = {}
-_VERIFY_PLAN_CACHE = bool(int(os.environ.get("RB200_VERIFY_PLAN_CACHE", "0")))
-
-
-def _remember_plan(pkey, fop, shards, bound, gred_out, gred_src):
-    """Keep the bound op list of a single-range, all-local flush as a template: the struct bytes, and for every pointer
-    in it the shard it points into and the byte offset from that shard's interior origin."""
-    import ctypes
-
-    vpatch = []
-    for v, b in enumerate(bound):
-        if len(b) < 4 or b[3] is None:
-            return  # (an operand that is not shard-addressed: not a plain local flush)
-        vpatch.append(b[0] - shards[v].ptr(0))
-    rpatch = []
-    if gred_out:
-        for slot, g in enumerate(gred_out):
-            if g is None or slot not in gred_src:
-                return
-            v = gred_src[slot]
-            rpatch.append((slot, v, g[0] - shards[v].ptr(0)))
-    if len(_plan_cache) >= 1024:
-        _plan_cache.clear()
-    _plan_cache[pkey] = ("single", ctypes.string_at(ctypes.addressof(fop), ctypes.sizeof(fop)), vpatch, rpatch)
-
-
-def _run_planned(plan, shards, verify_prog, views, exec_dist, gred):
-    template, vpatch, rpatch = plan
-    fop = cabi.FusedOp.from_buffer_copy(template)
-    fv = fop.views
-    for v, off in enumerate(vpatch):
-        sh = shards[v]
-        one = fv[v]
-        one.base = sh.ptr(0) + off
-        one.alloc_lo, one.alloc_hi = sh.bounds
-    for (slot, v, off) in rpatch:
-        fop.reds[slot].out = shards[v].ptr(0) + off
-    if fop.n_reds:
-        fop.red_scratch = RT.red_scratch().data_ptr()
-    if verify_prog is not None:
-        _verify_plan(fop, verify_prog, views, exec_dist, gred)
-    RT.submit(fop)
-
-
-def _verify_plan(fop, prog, views, exec_dist, gred):
-    """RB200_VERIFY_PLAN_CACHE=1: rebuild the bound op list the long way (without submitting it) and compare bytes."""
-    import ctypes
-
-    saved = dict(_plan_cache)
-    _plan_cache.clear()
-    captured = []
-    orig = RT.submit
-    RT.submit = lambda f: captured.append(f) or f
-    try:
-        _plan_cache_disabled.append(1)
-        run_deferred_ops("verify", views, prog, exec_dist, gred, [], None)
-    finally:
-        _plan_cache_disabled.pop()
-        RT.submit = orig
-        _plan_cache.clear()
-        _plan_cache.update(saved)
-    if len(captured) != 1:
-        raise AssertionError("flush-plan memo: the general path issues %d launches for a memoised single-range flush" % len(captured))
-    a = ctypes.string_at(ctypes.addressof(fop), ctypes.sizeof(fop))
-    b = ctypes.string_at(ctypes.addressof(captured[0]), ctypes.sizeof(captured[0]))
-    if a != b:
-        raise AssertionError("flush-plan memo: the patched template differs from a freshly bound op list")
-
-
-_plan_cache_disabled = []
+_plan_cache = {}  # flush key -> script (_FlushTape)
 
 
 class _FlushTape:
-    """Everything a flush of the general path does to the GPU and to the other ranks, as it is done AND as a script:
-    buffer allocations, launches (the bound rb200_fused_op with its pointers replaced by (resource, byte offset) pairs:
-    a resource is the shard of one of the flush's views or one of the buffers the flush allocated), the all-gather,
-    the grouped sends / receives, the points where the launching stream waits for them, the fold of axis partials.
-    A later flush with the same key (op list, partitions of the op and of every operand, shard layouts) replays the
-    script instead of planning again: pack -> P2P -> interior ranges -> wait -> boundary ranges becomes a loop over
-    prepared structs (`_replay_tape`).  RB200_VERIFY_PLAN_CACHE=1: every hit plans again and the new script must be
-    identical to the memoised one."""
+    """Everything a flush does to the GPU and to the other ranks, as it is done AND as a script: buffer allocations,
+    launches (the bound rb200_fused_op with its pointers replaced by (resource, byte offset) pairs: a resource is the
+    shard of one of the flush's views or one of the buffers the flush allocated), the all-gather, the grouped sends /
+    receives, the points where the launching stream waits for them, the fold of axis partials.  A later flush with the
+    same key (op list, partitions of the op and of every operand, shard layouts) replays the script instead of planning
+    again: pack -> P2P -> interior ranges -> wait -> boundary ranges becomes a loop over prepared structs
+    (`_replay_tape`); the plain flush (one range, all local) is a script of one launch.  RB200_VERIFY_PLAN_CACHE=1:
+    every hit plans again and the new script must be identical to the memoised one."""
 
     def __init__(self, shards):
         self.shards = shards
@@ -1109,13 +1040,13 @@ class _FlushTape:
 
     # ---- resources
     def _resolve(self, p):
-        """Device address -> (0, view index, byte offset from that shard's interior origin) | (1, buffer slot, offset)."""
+        """Device address -> (0, view index, byte offset from the start of that shard's buffer) | (1, buffer slot, offset)."""
         if not p:
             return None
         for i, sh in enumerate(self.shards):
             lo, hi = sh.bounds
             if lo <= p < hi:
-                return (0, i, p - sh.ptr(0))
+                return (0, i, p - lo)
         for k, b in enumerate(self.buffers):
             lo = b.data_ptr()
             if lo <= p < lo + builtins.max(1, b.numel() * b.element_size()):
@@ -1194,7 +1125,7 @@ class _FlushTape:
 def _addr(res, shards, bufs):
     kind, idx, off = res
     if kind == 0:
-        return shards[idx].ptr(0) + off
+        return shards[idx].bounds[0] + off
     if kind == 1:
         return bufs[idx].data_ptr() + off
     return RT.red_scratch().data_ptr()
@@ -1202,43 +1133,35 @@ def _addr(res, shards, bufs):
 
 def _submit_patched(action, shards, bufs):
     _, template, patches, rp, scratch = action
-    fop = cabi.FusedOp.from_buffer_copy(template)
-    fv = fop.views
-    for v, (res, bounded) in enumerate(patches):
-        one = fv[v]
-        one.base = _addr(res, shards, bufs)
-        if bounded:
-            one.alloc_lo, one.alloc_hi = shards[res[1]].bounds
-    for sl, res in enumerate(rp):
-        if res is not None:
-            fop.reds[sl].out = _addr(res, shards, bufs)
-    if scratch is not None:
-        fop.red_scratch = _addr(scratch, shards, bufs)
-    RT.submit(fop)
+    views = [(_addr(res, shards, bufs), shards[res[1]].bounds if bounded else None) for res, bounded in patches]
+    outs = [None if res is None else _addr(res, shards, bufs) for res in rp]
+    RT.submit(fill_template(template, views, outs, None if scratch is None else _addr(scratch, shards, bufs)))
 
 
 def _replay_tape(script, shards):
     """Run a memoised flush script against this flush's shards (see _FlushTape)."""
     import torch
-    import torch.distributed as dist
 
     actions, counts = script
     bufs = []
     works = []
-    dev = RT.device
     for a in actions:
         k = a[0]
         if k == "launch":
             _submit_patched(a, shards, bufs)
         elif k == "alloc":
-            bufs.append(torch.empty(a[1], dtype=a[2], device=dev))
+            bufs.append(torch.empty(a[1], dtype=a[2], device=RT.device))
         elif k == "p2p":
+            import torch.distributed as dist  # (only scripts that talk to other ranks pay for it)
+
             works += dist.batch_isend_irecv([dist.P2POp(dist.isend if s else dist.irecv, bufs[b].view(torch.uint8), peer) for (s, b, peer) in a[1]])
         elif k == "wait":
             for wk in works:
                 wk.wait()
             works = []
         elif k == "allgather":
+            import torch.distributed as dist
+
             works.append(dist.all_gather_into_tensor(bufs[a[1]].view(torch.uint8), bufs[a[2]].view(torch.uint8), async_op=True))
         else:  # fold
             RT._reduce_partials(_addr(a[1], shards, bufs), _addr(a[2], shards, bufs), a[3], a[4], a[5], a[6], a[7], RT.stream_handle())
@@ -1248,8 +1171,6 @@ def _replay_tape(script, shards):
     RT.collectives += counts[1]
     RT.ring_receives += counts[2]
     RT.keepalive = bufs
-
-
 
 
 def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
@@ -1268,39 +1189,28 @@ def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
         shards.append(sh)
     nviews = len(views)
     vdist = [det.distribution for (_, det) in views]
-    # ---- flush-plan memo: a flush whose operands are all local on every rank and that runs as ONE range without axis
-    # reductions is, apart from the buffer addresses, a function of (op list, distributions, shard layouts): the bound
-    # rb200_fused_op of the first execution is kept as a template and later executions only patch pointers into a copy
-    # Every other flush (several ranges, pieces exchanged with other ranks, an all-gathered operand, axis reductions) is
-    # recorded as a script of allocations / launches / transfers / waits with symbolic addresses (_FlushTape) and replayed.
-    pkey = None
-    verify_script = None
-    if not _plan_cache_disabled:
-        pkey = (prog, w, W, tuple([sv.key() for sv in exec_dist]), tuple([tuple([sv.key() for sv in vd]) for vd in vdist]),
-                tuple([(sh.shape, sh.border) for sh in shards]), tuple(red_axes) if red_axes else (),
-                # (what the ring of a padded block can receive depends on the partition of the whole array)
-                tuple([tuple([sv.key() for sv in bdarray.get_by_gid(g).distribution]) if sh.border else None
-                       for (g, _), sh in zip(views, shards)]) if W > 1 else ())
-        plan = _plan_cache.get(pkey)
-        if plan is not None:
-            if plan[0] == "single":
-                _run_planned(plan[1:], shards, prog if _VERIFY_PLAN_CACHE else None, views, exec_dist, gred)
-                return
-            if not _VERIFY_PLAN_CACHE:
-                _replay_tape(plan[1], shards)
-                return
-            verify_script = plan[1]
+    # ---- flush memo: apart from the buffer addresses, everything a flush does is a function of (op list, partitions of
+    # the op and of every operand, shard layouts).  The first execution is recorded as a script of allocations / launches
+    # / transfers / waits with symbolic addresses (_FlushTape); later executions replay it.
+    pkey = (prog, w, W, tuple([sv.key() for sv in exec_dist]), tuple([tuple([sv.key() for sv in vd]) for vd in vdist]),
+            tuple([(sh.shape, sh.border) for sh in shards]), tuple(red_axes) if red_axes else (),
+            # (what the ring of a padded block can receive depends on the partition of the whole array)
+            tuple([tuple([sv.key() for sv in bdarray.get_by_gid(g).distribution]) if sh.border else None
+                   for (g, _), sh in zip(views, shards)]) if W > 1 else ())
+    memo = _plan_cache.get(pkey)
+    if memo is not None and not _VERIFY_PLAN_CACHE:
+        _replay_tape(memo, shards)
+        return
     tape = _FlushTape(shards)
 
     def _done():
         script = tape.finish()
-        if verify_script is not None:
-            if script != verify_script:
-                raise AssertionError("flush-script memo: planning the same flush again gives a different script")
-        elif pkey is not None:
+        if memo is None:
             if len(_plan_cache) >= 1024:
                 _plan_cache.clear()
-            _plan_cache[pkey] = ("tape", script)
+            _plan_cache[pkey] = script
+        elif script != memo:
+            raise AssertionError("flush-script memo: planning the same flush again gives a different script")
     vcode = [rb_dtype(det.dtype) for (_, det) in views]
     written = [bool(prog.view_written.get(i)) for i in range(nviews)]
     ared_views = set()
@@ -1434,7 +1344,6 @@ def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
     red_axes = list(red_axes) if red_axes else []
     order = red_axes + [d for d in range(k) if d not in red_axes]
     gred_out = None
-    gred_src = {}
     if gred:
         gred_out = [None] * len(prog.reds)
         for (slot, red_view) in gred:
@@ -1442,7 +1351,6 @@ def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
             # this worker's element of the partial array: the first element of its (size-1) block
             off, _ = RT.bind_view(vdist[i][w], shards[i].strides, shardview.clean_range(vdist[i][w]))
             gred_out[slot] = (shards[i].ptr(off), vcode[i])
-            gred_src[slot] = i
     def _needs_transfer(r):
         for i in range(nviews):
             for (box, ptr, cst, sv, dep) in parts[i]:
@@ -1492,13 +1400,6 @@ def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
         shape_r = [int(x) for x in r.size]
         gs = [int(x) for x in r.start]
         if not ared:
-            if single and not pending and not post_wait and not tape.buffers and not tape.actions and len(ranges) == 1 \
-                    and verify_script is None:
-                # the plain flush: one launch, everything local - kept as a single template (see _remember_plan)
-                fop = RT.launch(prog, shape_r, gs, bound, reds=gred_out, worker_num=w, num_workers=W)
-                if pkey is not None:
-                    _remember_plan(pkey, fop, shards, bound, gred_out, gred_src)
-                return
             tape.launch(prog, shape_r, gs, bound, reds=gred_out, worker_num=w, num_workers=W)
             continue
         # ---- axis reduction: stage 1 into per-split partials, then fold into the partial array

@@ -262,20 +262,13 @@ class Runtime:
                n_axis_red, axis_nsplit, worker_num, num_workers)
         tpl = _launch_cache.get(key)
         if tpl is not None:
-            fop = cabi.FusedOp.from_buffer_copy(tpl)
-            fv = fop.views
-            for v, bv in enumerate(bound_views):
-                one = fv[v]
-                one.base = bv[0]
-                if len(bv) > 3 and bv[3] is not None:
-                    one.alloc_lo, one.alloc_hi = bv[3]
+            outs = scratch = None
             if program.reds:
                 if reds is not None:
-                    for sl, r in enumerate(reds):
-                        if r is not None:
-                            fop.reds[sl].out = r[0]
-                fop.red_scratch = axis_partials if n_axis_red else self.red_scratch().data_ptr()
-            if _VERIFY_LAUNCH_CACHE:
+                    outs = [None if r is None else r[0] for r in reds]
+                scratch = axis_partials if n_axis_red else self.red_scratch().data_ptr()
+            fop = fill_template(tpl, [(bv[0], bv[3] if len(bv) > 3 else None) for bv in bound_views], outs, scratch)
+            if _VERIFY_PLAN_CACHE:
                 fresh = self._build(program, rng_shape, gstart, bound_views, reds, n_axis_red, axis_nsplit, axis_partials, worker_num, num_workers)
                 if ctypes.string_at(ctypes.addressof(fop), ctypes.sizeof(fop)) != ctypes.string_at(ctypes.addressof(fresh), ctypes.sizeof(fresh)):
                     raise AssertionError("launch memo: the patched template differs from a freshly bound op list")
@@ -402,7 +395,29 @@ class Runtime:
             self.backend.synchronize()
 
 
+def fill_template(template, views, red_outs=None, red_scratch=None):
+    """A copy of the bytes of a bound rb200_fused_op with its addresses filled in.  views: (base, (alloc_lo, alloc_hi) or
+    None) per view; red_outs: the output address of every reduction slot, None keeping the template's; red_scratch: None
+    keeps the template's."""
+    fop = cabi.FusedOp.from_buffer_copy(template)
+    fv = fop.views
+    for v, (base, bounds) in enumerate(views):
+        one = fv[v]
+        one.base = base
+        if bounds is not None:
+            one.alloc_lo, one.alloc_hi = bounds
+    if red_outs:
+        for sl, out in enumerate(red_outs):
+            if out is not None:
+                fop.reds[sl].out = out
+    if red_scratch is not None:
+        fop.red_scratch = red_scratch
+    return fop
+
+
 _launch_cache = {}
-_VERIFY_LAUNCH_CACHE = bool(int(os.environ.get("RB200_VERIFY_PLAN_CACHE", "0")))
+# RB200_VERIFY_PLAN_CACHE=1: every hit of the launch memo (here) and of the flush memo (ramba.run_deferred_ops) is
+# checked against planning the same thing again
+_VERIFY_PLAN_CACHE = bool(int(os.environ.get("RB200_VERIFY_PLAN_CACHE", "0")))
 
 RT = Runtime()

@@ -129,7 +129,8 @@ def test_dtypes_are_part_of_the_key(verified_memo):
         assert got.dtype == exp.dtype and onp.array_equal(got, exp)
 
 
-# ---- the flush-plan memo (ramba.py::run_deferred_ops): bound op lists of single-range, all-local flushes are templates
+# ---- the flush memo (ramba.py::run_deferred_ops): every flush is recorded as a script, later flushes with the same key
+# replay it
 @pytest.fixture
 def verified_plans(oracle_engine, monkeypatch):
     from ramba_b200 import ramba
@@ -139,24 +140,24 @@ def verified_plans(oracle_engine, monkeypatch):
     return ramba
 
 
-def test_repeated_flush_is_served_by_the_plan_memo(verified_plans, monkeypatch):
+def test_repeated_flush_is_replayed_from_its_script(verified_plans, monkeypatch):
     import ramba_b200 as rb
 
     planned = []
-    orig = verified_plans._run_planned
+    orig = verified_plans._replay_tape
 
     def counted(*a, **k):
         planned.append(1)
         return orig(*a, **k)
 
-    monkeypatch.setattr(verified_plans, "_run_planned", counted)
+    monkeypatch.setattr(verified_plans, "_replay_tape", counted)
     x = onp.arange(5000, dtype=onp.float64) / 7.0
     A = rb.fromarray(x)
     U = rb.fromarray(onp.arange(20 * 30 * 40, dtype=onp.float32).reshape(20, 30, 40) % 17)
     V = rb.zeros((20, 30, 40), dtype=onp.float32)
     rb.sync()
-    for it in range(4):
-        planned.clear()
+
+    def step():
         B = rb.sin(A)
         D = B * B + rb.cos(A) ** 2
         rb.sync()
@@ -164,9 +165,22 @@ def test_repeated_flush_is_served_by_the_plan_memo(verified_plans, monkeypatch):
                                + U[1:-1, 1:-1, :-2] + U[1:-1, 1:-1, 2:] - 6.0 * U[1:-1, 1:-1, 1:-1])
         rb.sync()
         s = float((A * 2.0 + 1.0).sum())  # a global reduction: the reduction output pointer is patched as well
+        return D, s
+
+    monkeypatch.setattr(verified_plans, "_VERIFY_PLAN_CACHE", False)  # (the verification mode plans every hit again)
+    for it in range(4):
+        planned.clear()
+        D, s = step()
         assert len(planned) == (0 if it == 0 else 3), (it, len(planned))
         assert onp.allclose(D.asarray(), 1.0)
         assert s == float((x * 2.0 + 1.0).sum())
+    # verified: planning each of the three flushes again must give its memoised script
+    monkeypatch.setattr(verified_plans, "_VERIFY_PLAN_CACHE", True)
+    planned.clear()
+    D, s = step()
+    assert len(planned) == 0
+    assert onp.allclose(D.asarray(), 1.0)
+    assert s == float((x * 2.0 + 1.0).sum())
     u = onp.asarray(U.asarray())
     e = onp.zeros_like(u)
     e[1:-1, 1:-1, 1:-1] = (u[:-2, 1:-1, 1:-1] + u[2:, 1:-1, 1:-1] + u[1:-1, :-2, 1:-1] + u[1:-1, 2:, 1:-1] + u[1:-1, 1:-1, :-2]
@@ -174,22 +188,24 @@ def test_repeated_flush_is_served_by_the_plan_memo(verified_plans, monkeypatch):
     assert onp.array_equal(V.asarray(), e)
 
 
-def test_plan_memo_executes_once_and_follows_the_buffers(verified_plans):
+def test_plan_memo_executes_once_and_follows_the_buffers(verified_plans, monkeypatch):
     import ramba_b200 as rb
 
-    a = rb.fromarray(onp.zeros(1000))
-    for it in range(5):
-        a += 1.0  # in place: a flush executed twice (or against a stale buffer) would show
-        rb.sync()
-    assert onp.array_equal(a.asarray(), onp.full(1000, 5.0))
-    outs = []
-    for it in range(4):  # fresh result buffers every iteration, all alive at the end
-        outs.append(a * float(2) + 1.0)
-        rb.sync()
-    for o in outs:
-        assert onp.array_equal(o.asarray(), onp.full(1000, 11.0))
-    # same op list over another layout: different template
-    b = rb.fromarray(onp.ones((10, 100)))
-    c = b[:, 1:] * 2.0 + 1.0
-    d = b[:, :-1] * 2.0 + 1.0
-    assert onp.array_equal(c.asarray(), onp.full((10, 99), 3.0)) and onp.array_equal(d.asarray(), onp.full((10, 99), 3.0))
+    for verify in (False, True):  # hits replayed, then hits planned again and checked against the memoised scripts
+        monkeypatch.setattr(verified_plans, "_VERIFY_PLAN_CACHE", verify)
+        a = rb.fromarray(onp.zeros(1000))
+        for it in range(5):
+            a += 1.0  # in place: a flush executed twice (or against a stale buffer) would show
+            rb.sync()
+        assert onp.array_equal(a.asarray(), onp.full(1000, 5.0))
+        outs = []
+        for it in range(4):  # fresh result buffers every iteration, all alive at the end
+            outs.append(a * float(2) + 1.0)
+            rb.sync()
+        for o in outs:
+            assert onp.array_equal(o.asarray(), onp.full(1000, 11.0))
+        # same op list over another layout: different script
+        b = rb.fromarray(onp.ones((10, 100)))
+        c = b[:, 1:] * 2.0 + 1.0
+        d = b[:, :-1] * 2.0 + 1.0
+        assert onp.array_equal(c.asarray(), onp.full((10, 99), 3.0)) and onp.array_equal(d.asarray(), onp.full((10, 99), 3.0))
