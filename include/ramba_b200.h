@@ -40,7 +40,7 @@
 extern "C" {
 #endif
 
-#define RB200_ABI_VERSION 4
+#define RB200_ABI_VERSION 5
 
 #define RB200_MAX_DIMS 5     /* iteration dims after host-side collapsing            */
 #define RB200_MAX_VIEWS 16   /* distinct array views per fused op                    */
@@ -142,7 +142,35 @@ enum rb200_op {
   RB200_OP_MULADD = 52,  /* a + b*c                                                */
   RB200_OP_MULSUB = 53,  /* a - b*c                                                */
   RB200_OP_MULRSUB = 54, /* b*c - a                                                */
-  RB200_NUM_OPS = 55
+  RB200_OP_PHILOX = 55,  /* counter-based random draw: element value = f(a, key); see below      */
+  RB200_NUM_OPS = 56
+};
+
+/* RB200_OP_PHILOX: one element of a random draw, a pure function of (key, index), so that the values do not depend on
+ * how the array is partitioned, on the number of ranks or on what the draw is fused with.
+ *   a: the int64 global C-order linear index i of the element in the drawn array (IOTA, ACC or REG)
+ *   b: RB200_K_SCAL, the 64-bit key of the draw (the Python layer derives it as
+ *        key = splitmix64(splitmix64(seed) ^ draw_number)
+ *      where draw_number counts the draws made from one generator state since it was seeded)
+ *   c: RB200_K_SCAL, the bound n >= 1 of the integer form (ignored by the other forms)
+ *   imm: the output form (rb200_philox_form); ctype must be the form's class.
+ * Block: philox4x32_10(counter, key) is Philox4x32-10 (Salmon et al., SC'11, "Random123") with
+ *   key = (key_lo32, key_hi32) and counter = (j_lo32, j_hi32, 0, 0), giving words w0..w3; half h of the block is the
+ *   64-bit integer x_h = w_{2h} | w_{2h+1} << 32.  Counter 0, key 0 gives 6627e8d5 e169c58d bc57ac4c 9b00dbd8.
+ * Forms (j = the block element i reads):
+ *   UNIFORM64 (F64): j = i >> 1, x = x_{i & 1}, value (x >> 11) * 2^-53, in [0, 1)
+ *   UNIFORM32 (F32): j = i >> 2, w = w_{i & 3}, value (w >> 8) * 2^-24, in [0, 1)
+ *   NORMAL64  (F64): j = i >> 1, Box-Muller with every step rounded separately: u1 = 1 - (x_0 >> 11) * 2^-53 in (0, 1],
+ *                    u2 = (x_1 >> 11) * 2^-53, r = sqrt(-2 * log(u1)), t = 2*pi * u2; element 2j is r*cos(t), 2j+1 is
+ *                    r*sin(t).  log, sqrt, sin and cos are the CUDA double-precision functions (not bit-identical
+ *                    to a host libm: the last bits may differ)
+ *   INTEGER   (I64): j = i >> 1, x = x_{i & 1}, value mulhi64(x, n) in [0, n); P(v) differs from 1/n by at most
+ *                    1/2^64 (the bias of a multiply-shift reduction is below n / 2^64 overall)                          */
+enum rb200_philox_form {
+  RB200_PHILOX_UNIFORM64 = 0,
+  RB200_PHILOX_UNIFORM32 = 1,
+  RB200_PHILOX_NORMAL64 = 2,
+  RB200_PHILOX_INTEGER = 3
 };
 
 enum rb200_redop { RB200_RED_ADD = 0, RB200_RED_MUL = 1, RB200_RED_MIN = 2, RB200_RED_MAX = 3 };

@@ -13,6 +13,7 @@ from .ramba import *  # noqa: F401,F403
 from .ramba import (ndarray, bdarray, deferred_op, sync, arange, empty, zeros, ones, full, fromarray, fromfunction,  # noqa: F401
                     asarray, array, where, HANDLED_FUNCTIONS, fromarray_local, local_block_to_host, stencil, sstencil)
 from . import ramba as _ramba
+from . import random  # noqa: F401  (`import ramba_b200.random as random`, like ramba.random)
 
 globals().update(_ramba.api)  # abs/min/max/sum/all/any shadow the builtins like in the reference
 

@@ -10,7 +10,7 @@ raises.
 import ctypes as C
 import os
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 MAX_DIMS = 5
 MAX_VIEWS = 16
 MAX_SCALARS = 32
@@ -31,10 +31,12 @@ OPS = [
     "GT", "LT", "GE", "LE", "EQ", "NE", "LAND", "LOR", "LXOR", "BAND", "BOR", "BXOR", "SHL", "SHR",
     "ABS", "SQUARE", "SQRT", "SIN", "COS", "TAN", "SINH", "COSH", "TANH", "ASIN", "ACOS", "ATAN",
     "NEG", "EXP", "LOG", "ISFINITE", "ISINF", "ISNAN", "ISNEGINF", "ISPOSINF", "LNOT", "INVERT",
-    "WHERE", "CVT", "SINCOS", "RED", "CBRT", "MULADD", "MULSUB", "MULRSUB",
+    "WHERE", "CVT", "SINCOS", "RED", "CBRT", "MULADD", "MULSUB", "MULRSUB", "PHILOX",
 ]
 OP = {name: i for i, name in enumerate(OPS)}
 RED_ADD, RED_MUL, RED_MIN, RED_MAX = range(4)
+# output forms of PHILOX (imm)
+PHILOX_UNIFORM64, PHILOX_UNIFORM32, PHILOX_NORMAL64, PHILOX_INTEGER = range(4)
 
 
 class Insn(C.Structure):

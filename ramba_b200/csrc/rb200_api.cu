@@ -9,6 +9,7 @@
 
 #include "rb200_launch.h"
 #include "rb200_handlers.h"
+#include "rb200_rng.h"
 #include "rb200_stream.h"
 #include "rb200_tile.h"
 
@@ -148,12 +149,13 @@ static void assign_handlers(KParams& P, const rb200_fused_op* op, int set) {
 // ---- debugging aids (A/B measurements, bisecting a parity failure), read once: each takes a kernel family, the TMA
 // loader or the row tiling out of the selection, in the launch and in rb200_describe_plan alike
 struct KillSwitches {
-  bool no_tile, no_stream, no_mapred, no_terms, no_tma, no_row_mode;
+  bool no_tile, no_stream, no_mapred, no_terms, no_tma, no_row_mode, no_rng;
 };
 static const KillSwitches& kill_switches() {
   static const KillSwitches k = {getenv("RB200_NO_TILE_KERNEL") != nullptr,   getenv("RB200_NO_STREAM_KERNEL") != nullptr,
                                  getenv("RB200_NO_MAPRED_KERNEL") != nullptr, getenv("RB200_NO_TERMS_KERNEL") != nullptr,
-                                 getenv("RB200_NO_TMA") != nullptr,           getenv("RB200_NO_ROW_MODE") != nullptr};
+                                 getenv("RB200_NO_TMA") != nullptr,           getenv("RB200_NO_ROW_MODE") != nullptr,
+                                 getenv("RB200_NO_RNG") != nullptr};
   return k;
 }
 
@@ -204,6 +206,17 @@ static int validate(const rb200_fused_op* op, bool* empty) {
     if (I.mask_reg != RB200_NOSTORE && I.mask_reg >= op->n_regs) return fail("mask_reg out of range");
     if (I.op == RB200_OP_SINCOS && I.st2 >= op->n_regs) return fail("sincos st2 out of range");
     if (I.op == RB200_OP_RED && I.b_idx >= op->n_reds) return fail("reduction slot out of range");
+    if (I.op == RB200_OP_PHILOX) {
+      if (I.imm > RB200_PHILOX_INTEGER) return fail("philox: bad output form");
+      const int cls = I.imm == RB200_PHILOX_UNIFORM32 ? RB200_T_F32 : I.imm == RB200_PHILOX_INTEGER ? RB200_T_I64 : RB200_T_F64;
+      if (I.ctype != cls) return fail("philox: compute class does not match the output form");
+      if (I.a_kind != RB200_K_IOTA && I.a_kind != RB200_K_ACC && I.a_kind != RB200_K_REG) return fail("philox: the index must be an index, the accumulator or a register");
+      if (I.b_kind != RB200_K_SCAL) return fail("philox: the key must be a scalar");
+      if (I.imm == RB200_PHILOX_INTEGER) {
+        if (I.c_kind != RB200_K_SCAL) return fail("philox: the integer form needs a scalar bound");
+        if ((long long)op->scalars[I.c_idx] <= 0) return fail("philox: the bound must be positive");
+      }
+    }
   }
   for (int i = 0; i < op->n_views; ++i) {
     if (dtype_size(op->views[i].dtype) == 0) return fail("bad view dtype");
@@ -225,13 +238,14 @@ static int validate(const rb200_fused_op* op, bool* empty) {
   return 0;
 }
 
-enum PlanForm { FORM_NONE, FORM_TILE, FORM_STREAM, FORM_AXIS_AS_1D, FORM_AXIS_REDUCE, FORM_ELEMENTWISE };
+enum PlanForm { FORM_NONE, FORM_TILE, FORM_STREAM, FORM_AXIS_AS_1D, FORM_AXIS_REDUCE, FORM_ELEMENTWISE, FORM_RNG };
 
 // Which kernel runs one op list, and everything its launch needs.  One per call: nothing is shared between calls.
 struct Plan {
   PlanForm form;
   TilePlan tile;      // FORM_TILE
   StreamPlan stream;  // FORM_STREAM
+  RngPlan rng;        // FORM_RNG
   KParams k;          // the general interpreter forms
   long long blocks;   // the general interpreter forms: grid and dynamic shared memory
   size_t smem;
@@ -346,6 +360,11 @@ static void make_plan(const rb200_fused_op* op, int sms, Plan& pl) {
   const KillSwitches& ks = kill_switches();
   pl.form = FORM_NONE;
   pl.n_split = pl.n_written = 0;
+  // ---- a plain random draw (rb200_rng.cu): only op lists with a PHILOX instruction qualify
+  if (!ks.no_rng && plan_rng(op, sms, pl.rng)) {
+    pl.form = FORM_RNG;
+    return;
+  }
   // ---- specialised kernels first: float-arithmetic op lists over 2-D / 3-D boxes (shifted-view stencils with the
   // halo tile staged in shared memory by TMA, and N-d elementwise maps) run on the lean machine of rb200_tile.cu
   if (!ks.no_tile && plan_stencil_tile(op, sms, !ks.no_terms, !ks.no_tma, pl.tile)) {
@@ -535,6 +554,7 @@ static std::string launch_failure(const Plan& pl) {
       snprintf(buf, sizeof(buf), "stream kernel%s launch (blocks=%lld smem=%zu staged=%d depth=%d terms=%d)", T.P.mode == 1 ? " (columns)" : "", T.blocks,
                T.smem, T.P.n_staged, T.P.depth, T.P.n_terms);
     } break;
+    case FORM_RNG: snprintf(buf, sizeof(buf), "rng_fill_kernel launch (blocks=%lld)", pl.rng.blocks); break;
     case FORM_AXIS_AS_1D: return "vm_elementwise_kernel (axis-as-1-D) launch";
     case FORM_AXIS_REDUCE: return "vm_axis_reduce_kernel launch";
     default:
@@ -554,6 +574,7 @@ static int launch(Plan& pl, cudaStream_t stream) {
     case FORM_NONE: return 0;
     case FORM_TILE: e = launch_stencil_tile(pl.tile, stream); break;
     case FORM_STREAM: e = launch_stream(pl.stream, stream); break;
+    case FORM_RNG: e = launch_rng(pl.rng, stream); break;
     case FORM_AXIS_AS_1D: e = launch_vm_elementwise_ax1d(P, blocks, pl.smem, stream); break;
     case FORM_AXIS_REDUCE: e = launch_vm_axis_reduce(P, blocks, pl.smem, stream); break;
     case FORM_ELEMENTWISE:
@@ -581,6 +602,7 @@ static int launch(Plan& pl, cudaStream_t stream) {
 static std::string describe(const rb200_fused_op* op, const Plan& pl) {
   if (pl.form == FORM_TILE) return describe_stencil_tile(pl.tile);
   if (pl.form == FORM_STREAM) return describe_stream(pl.stream);
+  if (pl.form == FORM_RNG) return describe_rng(pl.rng);
   if (pl.form == FORM_NONE) return "kernel=none";
   const char* form = pl.form == FORM_ELEMENTWISE ? "elementwise" : pl.form == FORM_AXIS_AS_1D ? "axis_as_1d" : "axis_reduce";
   const char* tiling = pl.form != FORM_ELEMENTWISE || op->ndim == 1 ? "" : pl.k.row_chunks > 0 ? " tiling=row" : " tiling=flat";

@@ -9,6 +9,7 @@
 
 #include "rb200_vm.cuh"
 #include "rb200_handlers.h"
+#include "rb200_philox.h"
 
 namespace rb200 {
 
@@ -921,8 +922,35 @@ __device__ __forceinline__ void h_red(C& cx, const UInsn& I, u64 (&racc)[NS][AX 
   }
 }
 
+// PHILOX: every element computes the block it reads (rb200_philox.h) and keeps its own lane of it
+template <class R, int V, class C> __device__ __forceinline__ void finish_bits(C& cx, const UInsn& I, const u64 (&b)[V]) {
+  R r[V];
+#pragma unroll
+  for (int k = 0; k < V; ++k) r[k] = CT<R>::get(b[k]);
+  cx.template finish<R>(I, r);
+}
+template <int V, class C> __device__ __forceinline__ void exec_philox(C& cx, const UInsn& I) {
+  long long a[V];
+  cx.template fetch<long long>(I.a_kind(), I.a_idx(), a);
+  const u64 key = cx.P.scalars[I.b_idx()];
+  const u64 n = I.c_kind() == RB200_K_SCAL ? cx.P.scalars[I.c_idx()] : 1ull;
+  const unsigned form = I.imm();
+  u64 b[V];
+#pragma unroll
+  for (int k = 0; k < V; ++k) b[k] = philox_element_bits(a[k], key, n, form);
+  switch (I.ctype()) {
+    case RB200_T_F64: finish_bits<double, V>(cx, I, b); break;
+    case RB200_T_F32: finish_bits<float, V>(cx, I, b); break;
+    default: finish_bits<long long, V>(cx, I, b);
+  }
+}
+
 // the generic path of one instruction (any opcode, class and operand kinds)
 template <int V, bool AX, int NS, class C> __device__ __forceinline__ void generic_body(C& cx, const UInsn& I, u64 (&racc)[NS][AX ? V : 1]) {
+  if (I.op() == RB200_OP_PHILOX) {
+    exec_philox<V>(cx, I);
+    return;
+  }
   if (I.op() == RB200_OP_CVT) {
     switch (I.imm() & 0xff) {
       case RB200_T_F64: exec_cvt_from<double, V>(cx, I); break;

@@ -132,6 +132,9 @@ class Node:
         self.store2 = None  # SINCOS: view the parked half is stored to
 
 
+# result class of each PHILOX output form (imm)
+PHILOX_CLASS = {cabi.PHILOX_UNIFORM64: T_F64, cabi.PHILOX_UNIFORM32: T_F32, cabi.PHILOX_NORMAL64: T_F64, cabi.PHILOX_INTEGER: T_I64}
+
 _FLOAT_UNARY = {"sqrt", "sin", "cos", "tan", "sinh", "cosh", "tanh", "asin", "acos", "atan", "exp", "log", "cbrt"}
 _PRED_UNARY = {"isfinite", "isinf", "isnan", "isneginf", "isposinf", "lnot"}
 _CMP = {"gt", "lt", "ge", "le", "eq", "ne"}
@@ -329,6 +332,16 @@ class Lowering:
             if op == "tofloat":  # class of a "float" result dtype for an int operand (sin(int) etc.)
                 x = self.build(expr.args[0], resolve)
                 return self.coerce(x, T_F32 if x.cls == T_F32 else T_F64)
+            if op == "philox":
+                # E("philox", index, key[, bound], imm=form): one element of a random draw (include/ramba_b200.h)
+                cls = PHILOX_CLASS[expr.imm]
+                args = [self.coerce(self.build(expr.args[0], resolve), T_I64)]
+                for a in expr.args[1:]:
+                    tv = self.build(a, resolve)
+                    if tv.kind != "scal" or tv.cls != T_I64:
+                        raise ProgramError("philox: key and bound must be integer scalars")
+                    args.append(tv)
+                return self._node("philox", cls, cls, False, args, imm=expr.imm)
             if len(expr.args) == 2:
                 return self._binary(op, self.build(expr.args[0], resolve), self.build(expr.args[1], resolve))
             if len(expr.args) == 1:
