@@ -40,7 +40,7 @@
 extern "C" {
 #endif
 
-#define RB200_ABI_VERSION 5
+#define RB200_ABI_VERSION 6
 
 #define RB200_MAX_DIMS 5     /* iteration dims after host-side collapsing            */
 #define RB200_MAX_VIEWS 16   /* distinct array views per fused op                    */
@@ -262,6 +262,66 @@ int rb200_reduce_partials(void* out, const void* partials, int64_t n, int64_t k,
 int64_t rb200_cumulative_scratch_bytes(int64_t n_outer, int64_t len, int64_t n_inner);
 int rb200_cumulative(const void* src, void* dst, int32_t dtype, int64_t n_outer, int64_t len, int64_t n_inner,
                      int32_t redop, const void* carry_in, void* totals_out, void* scratch, void* stream);
+
+/* ---- integer-array indexing (a[idx], a[idx] = v): data movement at computed addresses ----------------------------------
+ * What it stands for in the reference: getitem_array_executor / setitem_array_executor (ramba/ramba.py:6429-6545,
+ * 6143-6297), which move one element at a time in Python.  The host computes `lin`, the C-order linear index of every
+ * addressed element within the view (int64, -1 for an element with an out-of-range coordinate); these entry points move
+ * the elements.  Semantics shared by all three:
+ *   - an entry of lin outside [0, view size) is added to *bad (a device uint64 counter, may be NULL when n == 0) and is
+ *     never read or written;
+ *   - everything is enqueued on `stream`, and nothing synchronises with the host;
+ *   - malformed arguments (elem_bytes not 1/2/4/8, ndim out of range, a null pointer with n > 0, a view outside its
+ *     [alloc_lo, alloc_hi), a route table that is not a grid or has too many ranks) are rejected with a reason through
+ *     rb200_last_error before any device query.                                                                        */
+#define RB200_MAX_ROUTE_RANKS 64  /* owners of a route table                                  */
+#define RB200_MAX_ROUTE_CELLS 64  /* cells of a route table (the product of the cells per dim)  */
+#define RB200_MAX_ROUTE_CUTS 40   /* cut points of a route table, all dims together            */
+
+/* An N-d view addressed by the C-order linear index of its elements: element (c0..c_{k-1}) lives at
+ * base + elem_bytes * sum(c_d * stride[d]).  Strides are in elements and may be negative or 0; a padded shard is a view
+ * with the padded block's strides.  [alloc_lo, alloc_hi) is the allocation the view lies in; when both are non-NULL the
+ * library checks the view's first and last reachable bytes against it.                                                  */
+typedef struct rb200_index_view {
+  void* base;
+  int32_t ndim;       /* 1..RB200_MAX_DIMS                                        */
+  int32_t elem_bytes; /* 1, 2, 4 or 8                                             */
+  int64_t shape[RB200_MAX_DIMS];
+  int64_t stride[RB200_MAX_DIMS];
+  const void* alloc_lo;
+  const void* alloc_hi;
+} rb200_index_view;
+
+/* out[i] = view[lin[i]], i < n (out is contiguous, elem_bytes per element).                                            */
+int rb200_gather(const rb200_index_view* view, const int64_t* lin, int64_t n, void* out, uint64_t* bad, void* stream);
+
+/* view[lin[i]] = values[i], i < n (values contiguous).  With duplicate entries in lin one of the values lands.         */
+int rb200_scatter(const rb200_index_view* view, const int64_t* lin, int64_t n, const void* values, uint64_t* bad, void* stream);
+
+/* The partition of a distributed view as a grid (host memory, read during the call).  Along dim d the view is cut at
+ * cuts[cut_start[d] .. cut_start[d] + n_cells[d]] (ascending, 0 first, shape[d] last); cell (j0..j_{k-1}) (C order over
+ * the cell grid) is held by rank cell_owner[cell], whose element (c0..) of the view lies at local element offset
+ * cell_offset[cell] + sum((c_d - cuts[cut_start[d] + j_d]) * cell_stride[cell * ndim + d]) of its shard.           */
+typedef struct rb200_route_table {
+  int32_t ndim;
+  int32_t n_ranks; /* 1..RB200_MAX_ROUTE_RANKS                                 */
+  int64_t shape[RB200_MAX_DIMS];
+  int32_t n_cells[RB200_MAX_DIMS];
+  int32_t cut_start[RB200_MAX_DIMS];
+  const int64_t* cuts;
+  const int32_t* cell_owner;
+  const int64_t* cell_offset;
+  const int64_t* cell_stride;
+} rb200_route_table;
+
+/* Route the requests lin[0..n) to the ranks that own them.  counts[r] (n_ranks entries) receives the number of valid
+ * requests owned by rank r; the requests are grouped by owner, rank 0's first, in the order of i inside each group, so the
+ * grouping is a pure function of the input: slots[i] is request i's position in that grouping (-1 for an out-of-range
+ * entry) and offsets[slots[i]] its owner's local element offset.  `scratch` holds rb200_route_scratch_bytes(n, n_ranks)
+ * bytes.                                                                                                              */
+int64_t rb200_route_scratch_bytes(int64_t n, int32_t n_ranks);
+int rb200_route(const rb200_route_table* table, const int64_t* lin, int64_t n, int64_t* offsets, int64_t* slots, int64_t* counts,
+                uint64_t* bad, void* scratch, void* stream);
 
 /* Which kernel rb200_run_deferred_ops would run `op` on and how (staged views, halos, TMA or cp.async loader, ring depth,
  * lean instructions, CTAs), as one text line in out[0..cap).  Needs no device and touches no pointer: the counterpart

@@ -10,7 +10,7 @@ raises.
 import ctypes as C
 import os
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 MAX_DIMS = 5
 MAX_VIEWS = 16
 MAX_SCALARS = 32
@@ -88,6 +88,30 @@ class FusedOp(C.Structure):
     ]
 
 
+class IndexView(C.Structure):
+    _fields_ = [
+        ("base", C.c_void_p),
+        ("ndim", C.c_int32), ("elem_bytes", C.c_int32),
+        ("shape", C.c_int64 * MAX_DIMS),
+        ("stride", C.c_int64 * MAX_DIMS),
+        ("alloc_lo", C.c_void_p),
+        ("alloc_hi", C.c_void_p),
+    ]
+
+
+class RouteTable(C.Structure):
+    _fields_ = [
+        ("ndim", C.c_int32), ("n_ranks", C.c_int32),
+        ("shape", C.c_int64 * MAX_DIMS),
+        ("n_cells", C.c_int32 * MAX_DIMS),
+        ("cut_start", C.c_int32 * MAX_DIMS),
+        ("cuts", C.c_void_p),
+        ("cell_owner", C.c_void_p),
+        ("cell_offset", C.c_void_p),
+        ("cell_stride", C.c_void_p),
+    ]
+
+
 assert C.sizeof(Insn) == 16
 
 # every symbol include/ramba_b200.h declares
@@ -103,6 +127,10 @@ EXPORTS = [
     "rb200_launch_count",
     "rb200_reset_launch_count",
     "rb200_device_sm_count",
+    "rb200_gather",
+    "rb200_scatter",
+    "rb200_route",
+    "rb200_route_scratch_bytes",
 ]
 
 _LIB = None
@@ -152,6 +180,15 @@ def load():
     lib.rb200_reset_launch_count.restype = None
     lib.rb200_device_sm_count.argtypes = []
     lib.rb200_device_sm_count.restype = C.c_int
+    lib.rb200_gather.argtypes = [C.POINTER(IndexView), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.rb200_gather.restype = C.c_int
+    lib.rb200_scatter.argtypes = [C.POINTER(IndexView), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.rb200_scatter.restype = C.c_int
+    lib.rb200_route.argtypes = [C.POINTER(RouteTable), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                C.c_void_p]
+    lib.rb200_route.restype = C.c_int
+    lib.rb200_route_scratch_bytes.argtypes = [C.c_int64, C.c_int32]
+    lib.rb200_route_scratch_bytes.restype = C.c_int64
     if lib.rb200_abi_version() != ABI_VERSION:
         raise CabiError("libramba_b200.so ABI %d != binding ABI %d: rebuild" % (lib.rb200_abi_version(), ABI_VERSION))
     _LIB = lib
@@ -205,3 +242,60 @@ def launch_count():
 
 def reset_launch_count():
     load().rb200_reset_launch_count()
+
+
+def index_view(base, shape, strides, elem_bytes, bounds=None):
+    """An IndexView struct: element (c0..) at base + elem_bytes * sum(c_d * strides[d]) (device addresses as ints)."""
+    v = IndexView()
+    v.base = base
+    v.ndim = len(shape)
+    v.elem_bytes = elem_bytes
+    for d, (n, s) in enumerate(zip(shape, strides)):
+        v.shape[d] = int(n)
+        v.stride[d] = int(s)
+    if bounds is not None:
+        v.alloc_lo, v.alloc_hi = bounds
+    return v
+
+
+def route_table(shape, cuts, owners, offsets, strides, n_ranks):
+    """A RouteTable struct over host arrays: cuts is a list (per dim) of ascending cut points, owners / offsets one entry
+    per cell (C order over the cell grid), strides ndim entries per cell.  Returns (struct, arrays to keep alive)."""
+    import numpy as np
+
+    k = len(shape)
+    flat_cuts = np.ascontiguousarray(np.concatenate([np.asarray(c, dtype=np.int64) for c in cuts]), dtype=np.int64)
+    own = np.ascontiguousarray(owners, dtype=np.int32)
+    off = np.ascontiguousarray(offsets, dtype=np.int64)
+    st = np.ascontiguousarray(np.asarray(strides, dtype=np.int64).reshape(-1))
+    t = RouteTable()
+    t.ndim = k
+    t.n_ranks = n_ranks
+    start = 0
+    for d in range(k):
+        t.shape[d] = int(shape[d])
+        t.n_cells[d] = len(cuts[d]) - 1
+        t.cut_start[d] = start
+        start += len(cuts[d])
+    t.cuts, t.cell_owner, t.cell_offset, t.cell_stride = flat_cuts.ctypes.data, own.ctypes.data, off.ctypes.data, st.ctypes.data
+    return t, (flat_cuts, own, off, st)
+
+
+def _p(x):
+    return C.c_void_p(x) if x else None
+
+
+def gather(view, lin, n, out, bad, stream=None):
+    check(load().rb200_gather(C.byref(view), _p(lin), n, _p(out), _p(bad), _p(stream)))
+
+
+def scatter(view, lin, n, values, bad, stream=None):
+    check(load().rb200_scatter(C.byref(view), _p(lin), n, _p(values), _p(bad), _p(stream)))
+
+
+def route(table, lin, n, offsets, slots, counts, bad, scratch, stream=None):
+    check(load().rb200_route(C.byref(table), _p(lin), n, _p(offsets), _p(slots), _p(counts), _p(bad), _p(scratch), _p(stream)))
+
+
+def route_scratch_bytes(n, n_ranks):
+    return int(load().rb200_route_scratch_bytes(n, n_ranks))

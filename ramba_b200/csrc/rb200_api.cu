@@ -9,6 +9,7 @@
 
 #include "rb200_launch.h"
 #include "rb200_handlers.h"
+#include "rb200_index.h"
 #include "rb200_rng.h"
 #include "rb200_stream.h"
 #include "rb200_tile.h"
@@ -612,6 +613,66 @@ static std::string describe(const rb200_fused_op* op, const Plan& pl) {
   return buf;
 }
 
+// ---- integer-array indexing: argument checks (before any device query, so that they hold on a machine without a GPU)
+static int check_index_view(const rb200_index_view* v, const char* who) {
+  const std::string w(who);
+  if (!v) return fail(w + ": null view");
+  if (v->elem_bytes != 1 && v->elem_bytes != 2 && v->elem_bytes != 4 && v->elem_bytes != 8) return fail(w + ": elem_bytes must be 1, 2, 4 or 8");
+  if (v->ndim < 1 || v->ndim > RB200_MAX_DIMS) return fail(w + ": ndim out of range");
+  long long size = 1, lo = 0, hi = 0;  // element offsets of the first and last reachable element
+  for (int d = 0; d < v->ndim; ++d) {
+    if (v->shape[d] < 0) return fail(w + ": negative shape");
+    size *= v->shape[d];
+    const long long reach = (v->shape[d] > 0 ? v->shape[d] - 1 : 0) * v->stride[d];
+    if (reach < 0) lo += reach;
+    else hi += reach;
+  }
+  if (size == 0) return 0;
+  if (!v->base) return fail(w + ": null view base pointer");
+  if (v->alloc_lo && v->alloc_hi) {
+    const char* b = (const char*)v->base;
+    if (b + lo * v->elem_bytes < (const char*)v->alloc_lo || b + (hi + 1) * v->elem_bytes > (const char*)v->alloc_hi)
+      return fail(w + ": view outside its allocation");
+  }
+  return 0;
+}
+
+static int check_route_table(const rb200_route_table* t, RouteParams* R) {
+  if (!t) return fail("route: null table");
+  if (t->ndim < 1 || t->ndim > RB200_MAX_DIMS) return fail("route: ndim out of range");
+  if (t->n_ranks < 1 || t->n_ranks > RB200_MAX_ROUTE_RANKS) return fail("route: too many ranks (or none)");
+  if (!t->cuts || !t->cell_owner || !t->cell_offset || !t->cell_stride) return fail("route: null table array");
+  R->ndim = t->ndim;
+  R->n_ranks = t->n_ranks;
+  R->size = 1;
+  long long n_cells = 1;
+  int n_cuts = 0;
+  for (int d = 0; d < t->ndim; ++d) {
+    if (t->shape[d] < 0) return fail("route: negative shape");
+    if (t->n_cells[d] < 1) return fail("route: not a grid (no cells along a dim)");
+    R->shape[d] = t->shape[d];
+    R->size *= t->shape[d];
+    n_cells *= t->n_cells[d];
+    R->n_cells[d] = t->n_cells[d];
+    R->cut_start[d] = n_cuts;
+    const int first = t->cut_start[d], m = t->n_cells[d] + 1;
+    if (first < 0 || n_cuts + m > RB200_MAX_ROUTE_CUTS) return fail("route: too many cut points");
+    if (n_cells > RB200_MAX_ROUTE_CELLS) return fail("route: too many cells");
+    for (int j = 0; j < m; ++j) R->cuts[n_cuts + j] = t->cuts[first + j];
+    if (R->cuts[n_cuts] != 0 || R->cuts[n_cuts + m - 1] != t->shape[d]) return fail("route: not a grid (cuts must run from 0 to the extent)");
+    for (int j = 1; j < m; ++j)
+      if (R->cuts[n_cuts + j] <= R->cuts[n_cuts + j - 1] && t->shape[d] > 0) return fail("route: not a grid (cuts must ascend)");
+    n_cuts += m;
+  }
+  for (long long c = 0; c < n_cells; ++c) {
+    if (t->cell_owner[c] < 0 || t->cell_owner[c] >= t->n_ranks) return fail("route: cell owner out of range");
+    R->owner[c] = t->cell_owner[c];
+    R->offset[c] = t->cell_offset[c];
+    for (int d = 0; d < t->ndim; ++d) R->stride[c * t->ndim + d] = t->cell_stride[c * t->ndim + d];
+  }
+  return 0;
+}
+
 extern "C" {
 
 const char* rb200_last_error(void) { return g_last_error.c_str(); }
@@ -662,6 +723,54 @@ int rb200_cumulative(const void* src, void* dst, int32_t dtype, int64_t n_outer,
   const cudaError_t e = launch_scan(src, dst, dtype, n_outer, len, n_inner, redop, carry_in, totals_out, scratch, sms, (cudaStream_t)stream_v, &supported);
   if (!supported) return fail("cumulative: unsupported dtype");
   if (e != cudaSuccess) return fail_cuda("scan kernel launch", e);
+  g_launches.fetch_add(1);
+  return 0;
+}
+
+int rb200_gather(const rb200_index_view* view, const int64_t* lin, int64_t n, void* out, uint64_t* bad, void* stream_v) {
+  if (const int rc = check_index_view(view, "gather")) return rc;
+  if (n < 0) return fail("gather: negative n");
+  if (n == 0) return 0;
+  if (!lin || !out || !bad) return fail("gather: null pointer");
+  const int sms = sm_count();
+  if (sms <= 0) return fail("no usable CUDA device (libramba_b200 has no CPU path)");
+  const cudaError_t e = launch_gather(collapse_index_view(*view), (const long long*)lin, n, out, (unsigned long long*)bad, sms, (cudaStream_t)stream_v);
+  if (e != cudaSuccess) return fail_cuda("gather kernel launch", e);
+  g_launches.fetch_add(1);
+  return 0;
+}
+
+int rb200_scatter(const rb200_index_view* view, const int64_t* lin, int64_t n, const void* values, uint64_t* bad, void* stream_v) {
+  if (const int rc = check_index_view(view, "scatter")) return rc;
+  if (n < 0) return fail("scatter: negative n");
+  if (n == 0) return 0;
+  if (!lin || !values || !bad) return fail("scatter: null pointer");
+  const int sms = sm_count();
+  if (sms <= 0) return fail("no usable CUDA device (libramba_b200 has no CPU path)");
+  const cudaError_t e =
+      launch_scatter(collapse_index_view(*view), (const long long*)lin, n, values, (unsigned long long*)bad, sms, (cudaStream_t)stream_v);
+  if (e != cudaSuccess) return fail_cuda("scatter kernel launch", e);
+  g_launches.fetch_add(1);
+  return 0;
+}
+
+int64_t rb200_route_scratch_bytes(int64_t n, int32_t n_ranks) {
+  if (n < 0 || n_ranks < 1) return 256;
+  return (int64_t)route_scratch_bytes(n, n_ranks);
+}
+
+int rb200_route(const rb200_route_table* table, const int64_t* lin, int64_t n, int64_t* offsets, int64_t* slots, int64_t* counts, uint64_t* bad,
+                void* scratch, void* stream_v) {
+  RouteParams R;
+  if (const int rc = check_route_table(table, &R)) return rc;
+  if (n < 0) return fail("route: negative n");
+  if (!counts || !scratch) return fail("route: null pointer");
+  if (n > 0 && (!lin || !offsets || !slots || !bad)) return fail("route: null pointer");
+  const int sms = sm_count();
+  if (sms <= 0) return fail("no usable CUDA device (libramba_b200 has no CPU path)");
+  const cudaError_t e = launch_route(R, (const long long*)lin, n, (long long*)offsets, (long long*)slots, (long long*)counts,
+                                     (unsigned long long*)bad, scratch, sms, (cudaStream_t)stream_v);
+  if (e != cudaSuccess) return fail_cuda("route kernel launch", e);
   g_launches.fetch_add(1);
   return 0;
 }

@@ -23,6 +23,7 @@ import weakref
 import numpy as np
 
 from . import _cabi as cabi
+from . import advindex
 from . import common
 from . import shardview
 from .common import dprint, timer, add_time
@@ -1841,6 +1842,8 @@ class ndarray:
             return ndarray(self.shape, base=self, distribution=self.distribution, local_border=0,
                            readonly=self.readonly, maskarray=m)
         index = self._plain_index(index)
+        if advindex.has_advanced(index):
+            return advindex.getitem(self, index)
         if builtins.any(i is None for i in index):
             # newaxis: slice without the None terms, then insert unit dims where they stood
             n_spec = builtins.sum(1 for i in index if i is not None and i is not Ellipsis)
@@ -1910,6 +1913,9 @@ class ndarray:
             return
         if not (isinstance(index, ndarray) and index.dtype == np.bool_):
             index = self._plain_index(index)
+            if advindex.has_advanced(index):
+                advindex.setitem(self, index, value)
+                return
             if builtins.any(i is Ellipsis for i in index) and not builtins.any(i is None for i in index):
                 pos = [j for j, i in enumerate(index) if i is Ellipsis][0]
                 index = index[:pos] + (slice(None),) * (self.ndim - (len(index) - 1)) + index[pos + 1:]

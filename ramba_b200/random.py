@@ -173,6 +173,24 @@ class _State:
         res = self.draw(size, cabi.PHILOX_INTEGER, np.int64, tail=tail, bound=n)
         return res if np.dtype(dtype) == np.int64 else res.astype(dtype)
 
+    def choice(self, a, size=None, replace=True, p=None):
+        """`a[integers(0, len(a), size)]` (a range when `a` is an int): one draw, the same bits at any rank count."""
+        if not replace:
+            raise NotImplementedError("choice(replace=False) is not supported (it needs a permutation)")
+        if p is not None:
+            raise NotImplementedError("choice(p=...) is not supported")
+        if isinstance(a, numbers.Integral):
+            return self.integers(0, int(a), size)
+        pool = a if isinstance(a, _r.ndarray) else np.asarray(a)
+        if pool.ndim != 1:
+            raise ValueError("choice: a must be an int or a 1-D array")
+        if len(pool) == 0:
+            raise ValueError("choice: a cannot be empty")
+        idx = self.integers(0, len(pool), size)
+        if size is None:
+            return pool[int(idx)]
+        return pool[idx] if isinstance(pool, _r.ndarray) else _r.fromarray(pool)[idx]
+
 
 _global = _State()
 
@@ -216,8 +234,13 @@ def randint(low, high=None, size=None, dtype=np.int64):
     return _global.integers(low, high, size, dtype)
 
 
+def choice(a, size=None, replace=True, p=None):
+    """Elements of the 1-D array `a` (or of range(a)) picked uniformly with replacement; see _State.choice."""
+    return _global.choice(a, size, replace, p)
+
+
 class Generator:
-    """`numpy.random.Generator` subset: random, normal, standard_normal, uniform, integers."""
+    """`numpy.random.Generator` subset: random, normal, standard_normal, uniform, integers, choice."""
 
     def __init__(self, seed=None):
         self._state = _State(seed)
@@ -243,6 +266,9 @@ class Generator:
             high = int(high) + 1
         return self._state.integers(low, high, size, dtype)
 
+    def choice(self, a, size=None, replace=True, p=None):
+        return self._state.choice(a, size, replace, p)
+
 
 def default_rng(seed=None):
     return Generator(seed)
@@ -250,9 +276,9 @@ def default_rng(seed=None):
 
 class RandomState:
     """`numpy.random.RandomState` subset: random, random_sample, rand, randn, uniform, normal, standard_normal,
-    randint.  Any other method raises NotImplementedError."""
+    randint, choice.  Any other method raises NotImplementedError."""
 
-    _METHODS = ("random", "random_sample", "rand", "randn", "uniform", "normal", "standard_normal", "randint", "seed")
+    _METHODS = ("random", "random_sample", "rand", "randn", "uniform", "normal", "standard_normal", "randint", "choice", "seed")
 
     def __init__(self, seed=None):
         self._state = _State(seed)
@@ -282,6 +308,9 @@ class RandomState:
 
     def randint(self, low, high=None, size=None, dtype=np.int64):
         return self._state.integers(low, high, size, dtype)
+
+    def choice(self, a, size=None, replace=True, p=None):
+        return self._state.choice(a, size, replace, p)
 
     def __getattr__(self, name):
         if name.startswith("_"):

@@ -60,6 +60,13 @@ class Shard:
         shape = self.shape = tuple([int(s) for s in shape])
         self.dtype = np.dtype(dtype)
         border = self.border = int(border)
+        self.strides, self.origin = Shard.layout(shape, border)  # origin: element offset of interior element (0, 0, ...)
+        p = buf.data_ptr()
+        self.bounds = (p, p + buf.numel() * buf.element_size())  # [alloc_lo, alloc_hi) handed to the C-ABI
+
+    @staticmethod
+    def layout(shape, border):
+        """(element strides, origin) of a block of `shape` grown by `border`: also what another rank's shard looks like."""
         lay = Shard._layouts.get((shape, border))
         if lay is None:
             st = []
@@ -71,9 +78,7 @@ class Shard:
             if len(Shard._layouts) >= 4096:
                 Shard._layouts.clear()
             lay = Shard._layouts[(shape, border)] = (strides, sum(border * x for x in strides))
-        self.strides, self.origin = lay  # origin: element offset of interior element (0, 0, ...)
-        p = buf.data_ptr()
-        self.bounds = (p, p + buf.numel() * buf.element_size())  # [alloc_lo, alloc_hi) handed to the C-ABI
+        return lay
 
     def ptr(self, off=0):
         """Device address of interior-relative element offset `off`."""
@@ -121,6 +126,20 @@ class CudaBackend:
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         cabi.cumulative(src_ptr, dst_ptr, code, n_outer, length, n_inner, redop, carry_in, totals_out, scratch.data_ptr(),
                         self.stream_handle())
+        return scratch
+
+    def gather(self, view, lin, n, out, bad):
+        """rb200_gather on the current stream: out[i] = view[lin[i]] (view: a cabi.IndexView)."""
+        cabi.gather(view, lin, n, out, bad, self.stream_handle())
+
+    def scatter(self, view, lin, n, values, bad):
+        """rb200_scatter on the current stream: view[lin[i]] = values[i]."""
+        cabi.scatter(view, lin, n, values, bad, self.stream_handle())
+
+    def route(self, table, lin, n, offsets, slots, counts, bad):
+        """rb200_route on the current stream; returns the scratch buffer (the caller keeps it alive)."""
+        scratch = torch.empty(cabi.route_scratch_bytes(n, table.n_ranks), dtype=torch.uint8, device=self.device)
+        cabi.route(table, lin, n, offsets, slots, counts, bad, scratch.data_ptr(), self.stream_handle())
         return scratch
 
     def init_process_group(self):
