@@ -20,10 +20,12 @@ import itertools
 import numbers
 
 import numpy as np
+import torch
 
 from . import _cabi as cabi
 from . import common
 from . import shardview
+from .flush import _local_shape
 from .program import E, Iota
 from .runtime import RT, Shard
 
@@ -192,8 +194,6 @@ def _itemsize(dtype):
 
 
 def _shard(nd):
-    from .ramba import _local_shape
-
     bd = nd.bdarray
     sh = RT.shards.get(nd.gid) or RT.create_array(nd.gid, _local_shape(bd.distribution, common.worker_num), bd.dtype, bd.pad)
     bd.remote_constructed = True
@@ -218,8 +218,6 @@ def _flat_shard_view(nd):
 
 def _route_table(nd):
     """The partition of view nd as a grid: every rank's box, its owner and where the owner keeps it."""
-    from .ramba import _local_shape
-
     bd = nd.bdarray
     shape = nd.shape
     boxes = []
@@ -256,29 +254,14 @@ def _needs_copy(nd):
 
 def _exchange_counts(counts):
     """counts: this rank's requests per owner (device int64, W entries) -> M[p][q] on the host, for every p."""
-    import torch
-    import torch.distributed as dist
-
     W = common.num_workers
     allc = torch.empty(W * W, dtype=torch.int64, device=RT.device)
-    dist.all_gather_into_tensor(allc, counts)
-    RT.collectives += 1
-    RT.bytes_sent += 8 * W * (W - 1)
+    RT.all_gather(allc, counts).wait()
     return allc.cpu().numpy().reshape(W, W)
-
-
-def _p2p(ops):
-    import torch.distributed as dist
-
-    if ops:
-        for wk in dist.batch_isend_irecv(ops):
-            wk.wait()
 
 
 def _route(nd, lin_ptr, n):
     """Route this rank's n requests on view nd: (offsets, slots, M, starts, keep)."""
-    import torch
-
     be = RT.be()
     W = common.num_workers
     table, keep = _route_table(nd)
@@ -296,8 +279,6 @@ def _route(nd, lin_ptr, n):
 
 def _gather(src, lin_nd, out):
     """out[i] = src[lin[i]] for this rank's block of lin / out."""
-    import torch
-
     be = RT.be()
     w, W = common.worker_num, common.num_workers
     lin_sh, out_sh = _shard(lin_nd), _shard(out)
@@ -315,18 +296,16 @@ def _gather(src, lin_nd, out):
     nv = int(M[w].sum())
     flat = _flat_shard_view(src)
     rep = torch.empty(max(nv * isz, 1), dtype=torch.uint8, device=RT.device)
-    import torch.distributed as dist
-
     ops, reqs = [], []
     for q in range(W):
         if q != w and M[w][q]:
-            ops.append(dist.P2POp(dist.isend, offs[starts[q]:starts[q] + M[w][q]], q))
-            RT.bytes_sent += 8 * int(M[w][q])
+            ops.append((True, offs[starts[q]:starts[q] + M[w][q]], q))
         if q != w and M[q][w]:
             req = torch.empty(int(M[q][w]), dtype=torch.int64, device=RT.device)
-            ops.append(dist.P2POp(dist.irecv, req, q))
+            ops.append((False, req, q))
             reqs.append((q, req))
-    _p2p(ops)
+    for wk in RT.p2p(ops):
+        wk.wait()
     if M[w][w]:  # this rank's own elements: straight into the reply buffer
         be.gather(flat, offs[starts[w]:].data_ptr(), int(M[w][w]), rep[starts[w] * isz:].data_ptr(), bad.data_ptr())
         RT.launches += 1
@@ -335,13 +314,13 @@ def _gather(src, lin_nd, out):
         r = torch.empty(req.numel() * isz, dtype=torch.uint8, device=RT.device)
         be.gather(flat, req.data_ptr(), req.numel(), r.data_ptr(), bad.data_ptr())
         RT.launches += 1
-        ops.append(dist.P2POp(dist.isend, r, q))
-        RT.bytes_sent += r.numel()
+        ops.append((True, r, q))
         served.append(r)
     for q in range(W):
         if q != w and M[w][q]:
-            ops.append(dist.P2POp(dist.irecv, rep[starts[q] * isz:(starts[q] + M[w][q]) * isz], q))
-    _p2p(ops)
+            ops.append((False, rep[starts[q] * isz:(starts[q] + M[w][q]) * isz], q))
+    for wk in RT.p2p(ops):
+        wk.wait()
     if n:
         be.gather(cabi.index_view(rep.data_ptr(), [nv], [1], isz), slots.data_ptr(), n, out_sh.ptr(0), bad.data_ptr())
         RT.launches += 1
@@ -350,8 +329,6 @@ def _gather(src, lin_nd, out):
 
 def _scatter(dst, lin_nd, vals):
     """dst[lin[i]] = vals[i] for this rank's block of lin / vals."""
-    import torch
-
     be = RT.be()
     w, W = common.worker_num, common.num_workers
     lin_sh, val_sh = _shard(lin_nd), _shard(vals)
@@ -371,21 +348,19 @@ def _scatter(dst, lin_nd, vals):
     if n:  # the values in slot order, grouped by owner
         be.scatter(cabi.index_view(packed.data_ptr(), [nv], [1], isz), slots.data_ptr(), n, val_sh.ptr(0), bad.data_ptr())
         RT.launches += 1
-    import torch.distributed as dist
-
     ops, got = [], []
     for q in range(W):
         if q != w and M[w][q]:
-            ops.append(dist.P2POp(dist.isend, offs[starts[q]:starts[q] + M[w][q]], q))
-            ops.append(dist.P2POp(dist.isend, packed[starts[q] * isz:(starts[q] + M[w][q]) * isz], q))
-            RT.bytes_sent += (8 + isz) * int(M[w][q])
+            ops.append((True, offs[starts[q]:starts[q] + M[w][q]], q))
+            ops.append((True, packed[starts[q] * isz:(starts[q] + M[w][q]) * isz], q))
         if q != w and M[q][w]:
             req = torch.empty(int(M[q][w]), dtype=torch.int64, device=RT.device)
             v = torch.empty(int(M[q][w]) * isz, dtype=torch.uint8, device=RT.device)
-            ops.append(dist.P2POp(dist.irecv, req, q))
-            ops.append(dist.P2POp(dist.irecv, v, q))
+            ops.append((False, req, q))
+            ops.append((False, v, q))
             got.append((req, v))
-    _p2p(ops)
+    for wk in RT.p2p(ops):
+        wk.wait()
     flat = _flat_shard_view(dst)
     if M[w][w]:
         be.scatter(flat, offs[starts[w]:].data_ptr(), int(M[w][w]), packed[starts[w] * isz:].data_ptr(), bad.data_ptr())

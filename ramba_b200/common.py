@@ -5,7 +5,7 @@ environment keeps working; flags that only make sense for Ray/MPI/Numba are acce
 
 Execution model: SPMD, one process per GPU, every rank runs the same driver program and owns
 division `rank` of every array (the reference's SPMD-under-MPI mode, ramba/ramba.py:3986-3993,
-10683-10690).  `num_workers` is the torch.distributed world size (1 without a launcher).
+10683-10690).  `num_workers` is the launcher's WORLD_SIZE (1 without a launcher).
 """
 import os
 import sys

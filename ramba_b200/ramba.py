@@ -21,14 +21,16 @@ import numbers
 import weakref
 
 import numpy as np
+import torch
 
 from . import _cabi as cabi
 from . import advindex
 from . import common
 from . import shardview
 from .common import dprint, timer, add_time
+from .flush import _combine_program, _contig_strides, _local_shape, _pack_program, _plan_cache, run_deferred_ops
 from .program import E, Iota, Lowering, ProgramError, ProgramLimit, TempVar, dtype_class, rb_dtype
-from .runtime import RT, _VERIFY_PLAN_CACHE, fill_template, torch_dtype
+from .runtime import ALLREDUCE_OP, RT, torch_dtype
 
 int64 = np.int64
 float64 = np.float64
@@ -896,582 +898,6 @@ def format_program(prog, views, shape):
 
 
 # =============================================================================================
-# executing a flush on this worker
-# =============================================================================================
-_pack_programs = {}
-
-
-def _pack_program(src_code, dst_code):
-    key = (src_code, dst_code)
-    if key not in _pack_programs:
-        lw = Lowering([src_code, dst_code])
-        lw.store(1, lw.read_view(0))
-        _pack_programs[key] = lw.finish()
-    return _pack_programs[key]
-
-
-_combine_programs = {}
-
-
-def _combine_program(red_code, acc_code, redop):
-    """red_view = red_view (op) partial  — applies stage-1 axis partials to the partial array."""
-    key = (red_code, acc_code, redop)
-    if key not in _combine_programs:
-        lw = Lowering([red_code, acc_code])
-        name = {cabi.RED_ADD: "add", cabi.RED_MUL: "mul", cabi.RED_MIN: "min", cabi.RED_MAX: "max"}[redop]
-        tv = lw.build(E(name, lw.read_view(0), lw.read_view(1)), None)
-        lw.store(0, tv)
-        _combine_programs[key] = lw.finish()
-    return _combine_programs[key]
-
-
-def _local_shape(bd_dist, w):
-    sv = bd_dist[w]
-    return tuple(int(x) for x in sv.size)
-
-
-def _contig_strides(shape, bcast):
-    st = [0] * len(shape)
-    acc = 1
-    for d in reversed(range(len(shape))):
-        if bcast[d]:
-            st[d] = 0
-        else:
-            st[d] = acc
-            acc *= int(shape[d])
-    return st, acc
-
-
-def _gatherable(vd, exec_dist, bc, vshape, W):
-    """Elements per rank if view distribution `vd` can be brought to every rank with one all-gather: every rank runs a
-    non-empty part of the iteration box, no rank holds what it needs, every rank needs every rank's WHOLE part, and the
-    parts are equal consecutive chunks along the outermost non-broadcast axis (so that rank order == C order).  All
-    ranks evaluate this on the same metadata, so they agree.  None otherwise."""
-    k = len(bc)
-    nb = [d for d in range(k) if not bc[d] and int(vshape[d]) > 1]
-    if not nb:
-        return None
-    a = nb[0]
-    m = None
-    for p in range(W):
-        part = vd[p]
-        ex = shardview.clean_range(exec_dist[p])
-        if shardview.is_empty(part) or shardview.is_empty(ex) or shardview.is_compat(ex, part):
-            return None
-        if builtins.any((int(part.axis_map[d]) < 0) != bc[d] for d in range(k)):
-            return None
-        for d in range(k):
-            if bc[d]:
-                continue
-            if d == a:
-                if m is None:
-                    m = int(part.size[d])
-                if int(part.size[d]) != m or int(part.start[d]) != p * m:
-                    return None
-            elif int(part.start[d]) != 0 or int(part.size[d]) != int(vshape[d]):
-                return None
-    # every rank's box must cover the whole operand along its non-broadcast axes
-    for j in range(W):
-        ex = shardview.clean_range(exec_dist[j])
-        for d in range(k):
-            if not bc[d] and (int(ex.start[d]) != 0 or int(ex.size[d]) != int(vshape[d])):
-                return None
-    n = m
-    for d in nb[1:]:
-        n *= int(vshape[d])
-    if m * W != int(vshape[a]) or n * W > (1 << 22):
-        return None
-    return n
-
-
-def _ring_receivable(bd_dist, vd, exec_dist, w, W, shard):
-    """True when every remote piece of view distribution `vd` this rank needs lies within `shard.border` elements of its
-    own block (in every dim), i.e. can be received into the ring of the padded block and then be addressed by this
-    rank's own shardview of the view, extended past its box (what LocalNdarray.getborder prepares,
-    ramba/ramba.py:1260-1322, regions from shardview.compute_from_border, ramba/shardview_array.py:1069-1136)."""
-    mine = vd[w]
-    if shardview.is_empty(mine):
-        return False
-    k = len(mine.size)
-    b = shard.border
-    for d in range(k):
-        if int(mine.axis_map[d]) < 0 or int(mine.steps[d]) < 1:
-            return False
-    for peer in range(W):
-        if peer == w:
-            continue
-        part = shardview.intersect(vd[peer], exec_dist[w])
-        if shardview.is_empty(part):
-            continue
-        theirs = vd[peer]
-        for d in range(k):
-            a = int(mine.axis_map[d])
-            st = int(mine.steps[d])
-            if int(theirs.axis_map[d]) != a or int(theirs.steps[d]) != st:
-                return False
-            lo = int(mine.base_offset[a]) + (int(part.start[d]) - int(mine.start[d])) * st  # my block coordinates
-            hi = lo + (int(part.size[d]) - 1) * st
-            if lo < -b or hi > shard.shape[a] - 1 + b:
-                return False
-            # the same element through the owner's addressing: both must name the same global coordinate
-            g_theirs = int(bd_dist[peer].start[a]) + int(theirs.base_offset[a]) + (int(part.start[d]) - int(theirs.start[d])) * st
-            if int(bd_dist[w].start[a]) + lo != g_theirs:
-                return False
-    return True
-
-
-_plan_cache = {}  # flush key -> script (_FlushTape)
-
-
-class _FlushTape:
-    """Everything a flush does to the GPU and to the other ranks, as it is done AND as a script: buffer allocations,
-    launches (the bound rb200_fused_op with its pointers replaced by (resource, byte offset) pairs: a resource is the
-    shard of one of the flush's views or one of the buffers the flush allocated), the all-gather, the grouped sends /
-    receives, the points where the launching stream waits for them, the fold of axis partials.  A later flush with the
-    same key (op list, partitions of the op and of every operand, shard layouts) replays the script instead of planning
-    again: pack -> P2P -> interior ranges -> wait -> boundary ranges becomes a loop over prepared structs
-    (`_replay_tape`); the plain flush (one range, all local) is a script of one launch.  RB200_VERIFY_PLAN_CACHE=1:
-    every hit plans again and the new script must be identical to the memoised one."""
-
-    def __init__(self, shards):
-        self.shards = shards
-        self.actions = []
-        self.buffers = []
-        self.counts = [0, 0, 0]  # bytes sent, collectives, ring receives
-
-    # ---- resources
-    def _resolve(self, p):
-        """Device address -> (0, view index, byte offset from the start of that shard's buffer) | (1, buffer slot, offset)."""
-        if not p:
-            return None
-        for i, sh in enumerate(self.shards):
-            lo, hi = sh.bounds
-            if lo <= p < hi:
-                return (0, i, p - lo)
-        for k, b in enumerate(self.buffers):
-            lo = b.data_ptr()
-            if lo <= p < lo + builtins.max(1, b.numel() * b.element_size()):
-                return (1, k, p - lo)
-        if p == RT.red_scratch().data_ptr():
-            return (2, 0, 0)
-        raise ProgramError("internal: a bound pointer belongs to no shard or buffer of this flush")
-
-    def empty(self, n, dtype):
-        import torch
-
-        t = torch.empty(n, dtype=dtype, device=RT.device)
-        self.actions.append(("alloc", int(n), dtype))
-        self.buffers.append(t)
-        return t
-
-    def launch(self, *args, **kw):
-        fop = RT.launch(*args, submit=False, **kw)
-        patches = []
-        for v in range(fop.n_views):
-            one = fop.views[v]
-            patches.append((self._resolve(one.base), one.alloc_lo is not None and one.alloc_lo != 0))
-            one.base = 0
-            one.alloc_lo = 0
-            one.alloc_hi = 0
-        rp = []
-        for sl in range(fop.n_reds):
-            rp.append(self._resolve(fop.reds[sl].out))
-            fop.reds[sl].out = 0
-        scratch = self._resolve(fop.red_scratch)
-        fop.red_scratch = 0
-        import ctypes
-
-        self.actions.append(("launch", ctypes.string_at(ctypes.addressof(fop), ctypes.sizeof(fop)), tuple(patches), tuple(rp), scratch))
-        _submit_patched(self.actions[-1], self.shards, self.buffers)
-
-    def all_gather(self, full, mine):
-        import torch
-        import torch.distributed as dist
-
-        self.actions.append(("allgather", self._slot(full), self._slot(mine)))
-        return dist.all_gather_into_tensor(full.view(torch.uint8), mine.view(torch.uint8), async_op=True)
-
-    def _slot(self, t):
-        for k, b in enumerate(self.buffers):
-            if b is t:
-                return k
-        raise ProgramError("internal: a transfer buffer the flush did not allocate")
-
-    def p2p(self, ops):
-        """ops: [(is_send, buffer, peer)] -> the works of ONE grouped launch."""
-        import torch
-        import torch.distributed as dist
-
-        self.actions.append(("p2p", tuple([(bool(s), self._slot(b), int(peer)) for (s, b, peer) in ops])))
-        return dist.batch_isend_irecv([dist.P2POp(dist.isend if s else dist.irecv, b.view(torch.uint8), peer) for (s, b, peer) in ops])
-
-    def wait(self, works):
-        if works:
-            self.actions.append(("wait",))
-            for wk in works:
-                wk.wait()  # the launching stream waits for the transfers; the host does not
-
-    def reduce_partials(self, out_ptr, in_ptr, n, k, stride_k, code, rop):
-        self.actions.append(("fold", self._resolve(out_ptr), self._resolve(in_ptr), int(n), int(k), int(stride_k), int(code), int(rop)))
-        RT._reduce_partials(out_ptr, in_ptr, n, k, stride_k, code, rop, RT.stream_handle())
-
-    def finish(self):
-        RT.bytes_sent += self.counts[0]
-        RT.collectives += self.counts[1]
-        RT.ring_receives += self.counts[2]
-        RT.keepalive = self.buffers  # consumed on the launching stream; kept until the next flush
-        return (tuple(self.actions), tuple(self.counts))
-
-
-def _addr(res, shards, bufs):
-    kind, idx, off = res
-    if kind == 0:
-        return shards[idx].bounds[0] + off
-    if kind == 1:
-        return bufs[idx].data_ptr() + off
-    return RT.red_scratch().data_ptr()
-
-
-def _submit_patched(action, shards, bufs):
-    _, template, patches, rp, scratch = action
-    views = [(_addr(res, shards, bufs), shards[res[1]].bounds if bounded else None) for res, bounded in patches]
-    outs = [None if res is None else _addr(res, shards, bufs) for res in rp]
-    RT.submit(fill_template(template, views, outs, None if scratch is None else _addr(scratch, shards, bufs)))
-
-
-def _replay_tape(script, shards):
-    """Run a memoised flush script against this flush's shards (see _FlushTape)."""
-    import torch
-
-    actions, counts = script
-    bufs = []
-    works = []
-    for a in actions:
-        k = a[0]
-        if k == "launch":
-            _submit_patched(a, shards, bufs)
-        elif k == "alloc":
-            bufs.append(torch.empty(a[1], dtype=a[2], device=RT.device))
-        elif k == "p2p":
-            import torch.distributed as dist  # (only scripts that talk to other ranks pay for it)
-
-            works += dist.batch_isend_irecv([dist.P2POp(dist.isend if s else dist.irecv, bufs[b].view(torch.uint8), peer) for (s, b, peer) in a[1]])
-        elif k == "wait":
-            for wk in works:
-                wk.wait()
-            works = []
-        elif k == "allgather":
-            import torch.distributed as dist
-
-            works.append(dist.all_gather_into_tensor(bufs[a[1]].view(torch.uint8), bufs[a[2]].view(torch.uint8), async_op=True))
-        else:  # fold
-            RT._reduce_partials(_addr(a[1], shards, bufs), _addr(a[2], shards, bufs), a[3], a[4], a[5], a[6], a[7], RT.stream_handle())
-    for wk in works:
-        wk.wait()
-    RT.bytes_sent += counts[0]
-    RT.collectives += counts[1]
-    RT.ring_receives += counts[2]
-    RT.keepalive = bufs
-
-
-def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
-    """This worker's share of one flush (RemoteState.run_deferred_ops, ramba/ramba.py:3493-3819)."""
-    import torch
-
-    w, W = common.worker_num, common.num_workers
-    subspace = shardview.clean_range(exec_dist[w])
-    # allocate shards on first touch
-    shards = []
-    for (gid, det) in views:
-        bd = bdarray.get_by_gid(gid)
-        sh = RT.shards.get(gid)
-        if sh is None:
-            sh = RT.create_array(gid, _local_shape(bd.distribution, w), bd.dtype, bd.pad)
-        shards.append(sh)
-    nviews = len(views)
-    vdist = [det.distribution for (_, det) in views]
-    # ---- flush memo: apart from the buffer addresses, everything a flush does is a function of (op list, partitions of
-    # the op and of every operand, shard layouts).  The first execution is recorded as a script of allocations / launches
-    # / transfers / waits with symbolic addresses (_FlushTape); later executions replay it.
-    pkey = (prog, w, W, tuple([sv.key() for sv in exec_dist]), tuple([tuple([sv.key() for sv in vd]) for vd in vdist]),
-            tuple([(sh.shape, sh.border) for sh in shards]), tuple(red_axes) if red_axes else (),
-            # (what the ring of a padded block can receive depends on the partition of the whole array)
-            tuple([tuple([sv.key() for sv in bdarray.get_by_gid(g).distribution]) if sh.border else None
-                   for (g, _), sh in zip(views, shards)]) if W > 1 else ())
-    memo = _plan_cache.get(pkey)
-    if memo is not None and not _VERIFY_PLAN_CACHE:
-        _replay_tape(memo, shards)
-        return
-    tape = _FlushTape(shards)
-
-    def _done():
-        script = tape.finish()
-        if memo is None:
-            if len(_plan_cache) >= 1024:
-                _plan_cache.clear()
-            _plan_cache[pkey] = script
-        elif script != memo:
-            raise AssertionError("flush-script memo: planning the same flush again gives a different script")
-    vcode = [rb_dtype(det.dtype) for (_, det) in views]
-    written = [bool(prog.view_written.get(i)) for i in range(nviews)]
-    ared_views = set()
-    # which views are aligned with the iteration box on every worker?
-    local_everywhere = []
-    clean_exec = [shardview.clean_range(exec_dist[j]) for j in range(W)]
-    for i in range(nviews):
-        ok = True
-        if vdist[i] is not exec_dist:  # (the common case: the operand's distribution IS the op's)
-            for j in range(W):
-                ss = clean_exec[j]
-                if shardview.is_empty(ss):
-                    continue
-                if not shardview.is_compat(ss, vdist[i][j]):
-                    ok = False
-                    break
-        local_everywhere.append(ok)
-    # parts[i] = list of (box, data_ptr, elem_strides or None(shard-addressed), sv)
-    parts = [[] for _ in range(nviews)]
-    gathered = set()         # views served whole by an all-gathered buffer
-    ring = [False] * nviews  # views whose remote pieces are received into the ring of this rank's padded block
-    post_wait = []           # unpack launches that need the received data: (program, shape, bound views)
-    pending = []  # collectives / transfers in flight: waited for only before the first range that reads what they bring
-    if W > 1 and not builtins.all(local_everywhere):
-        RT.ensure_process_group()
-        import torch.distributed as dist
-
-        ops = []
-        for i in range(nviews):
-            if local_everywhere[i]:
-                continue
-            if written[i]:
-                raise ProgramError("fused op writes a view that is not aligned with its iteration space")
-            bc = [int(a) < 0 for a in vdist[i][0].axis_map]
-            ring[i] = shards[i].border > 0 and not shardview.is_empty(subspace) and _ring_receivable(
-                bdarray.get_by_gid(views[i][0]).distribution, vdist[i], exec_dist, w, W, shards[i])
-            itemsize = np.dtype(views[i][1].dtype).itemsize
-            g = _gatherable(vdist[i], exec_dist, bc, views[i][1].shape, W)
-            if g is not None:
-                # every rank needs every rank's part of this (small) operand and the parts are equal consecutive
-                # chunks: ONE all-gather into a buffer that then serves the whole iteration box as a single source
-                # (the reference ships W*(W-1) pickled pieces, ramba/ramba.py:3646-3693)
-                n = g
-                tdt = torch_dtype(views[i][1].dtype)
-                mine = tape.empty(n, tdt)
-                part = shardview.clean_range(vdist[i][w])
-                shp = [1 if bc[d] else int(part.size[d]) for d in range(len(bc))]
-                cst, _ = _contig_strides(shp, bc)
-                off, st = RT.bind_view(vdist[i][w], shards[i].strides, part)
-                tape.launch(_pack_program(vcode[i], vcode[i]), shp, [0] * len(shp),
-                            [(shards[i].ptr(off), [0 if bc[d] else st[d] for d in range(len(bc))], vcode[i]),
-                             (mine.data_ptr(), cst, vcode[i])])
-                full = tape.empty(W * n, tdt)
-                pending.append(tape.all_gather(full, mine))
-                tape.counts[0] += n * itemsize * (W - 1)
-                tape.counts[1] += 1
-                vshape = views[i][1].shape
-                fshape = [1 if bc[d] else int(vshape[d]) for d in range(len(bc))]
-                fst, _ = _contig_strides(fshape, bc)
-                box = shardview.ShardView(np.array([int(subspace.size[d]) if bc[d] else int(vshape[d]) for d in range(len(bc))], dtype=np.int64),
-                                          np.array([int(subspace.start[d]) if bc[d] else 0 for d in range(len(bc))], dtype=np.int64))
-                parts[i].append((box, full.data_ptr(), fst, None, True))
-                gathered.add(i)
-                continue
-            for peer in range(W):
-                if peer == w:
-                    continue
-                # what `peer` needs from me
-                pe = shardview.clean_range(exec_dist[peer])
-                if not shardview.is_empty(pe) and not shardview.is_compat(pe, vdist[i][peer]):
-                    part = shardview.intersect(vdist[i][w], exec_dist[peer])
-                    if not shardview.is_empty(part):
-                        shp = [1 if bc[d] else int(part.size[d]) for d in range(len(bc))]
-                        cst, n = _contig_strides(shp, bc)
-                        buf = tape.empty(max(n, 1), torch_dtype(views[i][1].dtype))
-                        off, st = RT.bind_view(vdist[i][w], shards[i].strides, part)
-                        src_ptr = shards[i].ptr(off)
-                        tape.launch(_pack_program(vcode[i], vcode[i]), shp, [0] * len(shp),
-                                    [(src_ptr, [0 if bc[d] else st[d] for d in range(len(bc))], vcode[i]),
-                                     (buf.data_ptr(), cst, vcode[i])])
-                        ops.append((True, buf, peer))
-                        tape.counts[0] += buf.numel() * buf.element_size()
-                # what I need from `peer`
-                if not shardview.is_empty(subspace) and not shardview.is_compat(subspace, vdist[i][w]):
-                    part = shardview.intersect(vdist[i][peer], exec_dist[w])
-                    if not shardview.is_empty(part):
-                        shp = [1 if bc[d] else int(part.size[d]) for d in range(len(bc))]
-                        cst, n = _contig_strides(shp, bc)
-                        buf = tape.empty(max(n, 1), torch_dtype(views[i][1].dtype))
-                        ops.append((False, buf, peer))
-                        pb = shardview.clean_range(part)
-                        if ring[i]:
-                            # getborder (ramba/ramba.py:1260-1322): the neighbour's edge lands in the ring of MY padded
-                            # block, where my own shardview of this view, extended past its box, addresses it
-                            off, st = RT.bind_view(vdist[i][w], shards[i].strides, pb)
-                            post_wait.append((_pack_program(vcode[i], vcode[i]), shp,
-                                              [(buf.data_ptr(), cst, vcode[i]), (shards[i].ptr(off), st, vcode[i])]))
-                            parts[i].append((pb, None, None, vdist[i][w], True))
-                            tape.counts[2] += 1
-                        else:
-                            parts[i].append((pb, buf.data_ptr(), cst, None, True))
-        if ops:
-            # the pack kernels run on the current stream; NCCL orders its transfers after them.  The transfers are NOT
-            # waited for here: ranges whose operands are all local (the interior of a stencil) are launched first and
-            # overlap with them (the reference sends, then blocks in the receive loop, ramba/ramba.py:3646-3693)
-            pending += tape.p2p(ops)
-    if shardview.is_empty(subspace):
-        tape.wait(pending)
-        _done()
-        return
-    # local parts
-    for i in range(nviews):
-        if i in gathered:
-            continue
-        sv = vdist[i][w]
-        if local_everywhere[i] or shardview.is_compat(subspace, sv):
-            parts[i].append((subspace, None, None, sv, False))
-        else:
-            part = shardview.intersect(sv, exec_dist[w])
-            if not shardview.is_empty(part):
-                parts[i].append((shardview.clean_range(part), None, None,
-                                 sv if ring[i] else shardview.mapslice_keep(sv, part.start, part.start + part.size), False))
-    # ranges: every operand has one source inside a range
-    single = builtins.all(len(p) == 1 and not p[0][4] and (p[0][0] is subspace or shardview.is_compat(p[0][0], subspace)) for p in parts)
-    if single:
-        ranges = [subspace]
-    else:
-        ranges = shardview.get_range_splits_list([shardview.clean_range(subspace)] + [p[0] for pl in parts for p in pl])
-        ranges = [r for r in ranges if not shardview.is_empty(r) and shardview.contains(subspace, r)]
-    k = len(subspace.size)
-    red_axes = list(red_axes) if red_axes else []
-    order = red_axes + [d for d in range(k) if d not in red_axes]
-    gred_out = None
-    if gred:
-        gred_out = [None] * len(prog.reds)
-        for (slot, red_view) in gred:
-            i = [j for j, (g, det) in enumerate(views) if g == red_view.gid and shardview.dist_is_eq(det.distribution, red_view.distribution)][0]
-            # this worker's element of the partial array: the first element of its (size-1) block
-            off, _ = RT.bind_view(vdist[i][w], shards[i].strides, shardview.clean_range(vdist[i][w]))
-            gred_out[slot] = (shards[i].ptr(off), vcode[i])
-    def _needs_transfer(r):
-        for i in range(nviews):
-            for (box, ptr, cst, sv, dep) in parts[i]:
-                if shardview.contains(box, r):
-                    if dep:
-                        return True
-                    break
-        return False
-
-    if pending:
-        ranges = sorted(ranges, key=lambda r: 1 if _needs_transfer(r) else 0)  # (stable: local ranges first)
-    for r in ranges:
-        if pending and _needs_transfer(r):
-            tape.wait(pending)  # the launching stream waits for the transfers; the host does not
-            pending = []
-            for (pp, pshape, pbound) in post_wait:
-                tape.launch(pp, pshape, [0] * len(pshape), pbound)
-            post_wait = []
-        bound = []
-        ok = True
-        for i in range(nviews):
-            src = None
-            if single:
-                src = parts[i][0]
-            else:
-                for (box, ptr, cst, sv, dep) in parts[i]:
-                    if shardview.contains(box, r):
-                        src = (box, ptr, cst, sv, dep)
-                        break
-            if src is None:
-                if ared and builtins.any(views[i][0] == rv.gid for (_, rv, _) in ared):
-                    src = None
-                ok = ok and (src is not None)
-                bound.append(None)
-                continue
-            box, ptr, cst, sv, dep = src
-            if sv is not None:
-                off, st = RT.bind_view(sv, shards[i].strides, r)
-                bound.append((shards[i].ptr(off), st, vcode[i], shards[i].bounds))
-            else:
-                off = 0
-                for d in range(k):
-                    off += int(r.start[d] - box.start[d]) * cst[d]
-                bound.append((ptr + off * np.dtype(views[i][1].dtype).itemsize, list(cst), vcode[i]))
-        if not ok:
-            raise ProgramError("internal: an operand has no source for range %r" % (r,))
-        shape_r = [int(x) for x in r.size]
-        gs = [int(x) for x in r.start]
-        if not ared:
-            tape.launch(prog, shape_r, gs, bound, reds=gred_out, worker_num=w, num_workers=W)
-            continue
-        # ---- axis reduction: stage 1 into per-split partials, then fold into the partial array
-        shape_p = [shape_r[d] for d in order]
-        gs_p = [gs[d] for d in order]
-        bound_p = [(b[0], [b[1][d] for d in order], b[2]) + tuple(b[3:]) for b in bound]
-        nred = len(red_axes)
-        kept_elems = 1
-        for d in range(nred, k):
-            kept_elems *= shape_p[d]
-        red_len = 1
-        for d in range(nred):
-            red_len *= shape_p[d]
-        kept_work = max(1, kept_elems // 4)
-        target = 132 * 2048  # H100 SXM: 132 SMs x 2048 resident threads
-        nsplit = 1 if kept_work >= target else builtins.min(builtins.max(1, red_len // 8), -(-target // kept_work))
-        nslots = len(prog.reds)
-        partials = tape.empty(nslots * nsplit * kept_elems + 1, torch.float64)
-        prog_p = _remap_iota(prog, order)
-        tape.launch(prog_p, shape_p, gs_p, bound_p, n_axis_red=nred, axis_nsplit=nsplit,
-                    axis_partials=partials.data_ptr(), worker_num=w, num_workers=W)
-        for (slot, red_view, redop) in ared:
-            rop, rct = prog.reds[slot]
-            acc_code = cabi.F64 if rct == cabi.T_F64 else cabi.I64
-            base = partials.data_ptr() + slot * nsplit * kept_elems * 8
-            tot_ptr = base
-            if nsplit > 1:
-                tot = tape.empty(kept_elems + 1, torch.float64)
-                tape.reduce_partials(tot.data_ptr(), base, kept_elems, nsplit, kept_elems, acc_code, rop)
-                tot_ptr = tot.data_ptr()
-            i = [j for j, (g, det) in enumerate(views) if g == red_view.gid and shardview.dist_is_eq(det.distribution, red_view.distribution)][0]
-            kept_shape = shape_p[nred:]
-            cst, _ = _contig_strides(kept_shape, [False] * len(kept_shape))
-            rb = bound_p[i]
-            tape.launch(_combine_program(vcode[i], acc_code, rop), kept_shape, gs_p[nred:],
-                        [(rb[0], rb[1][nred:], rb[2]), (tot_ptr, cst, acc_code)])
-    tape.wait(pending)  # (nothing needed them, e.g. an empty boundary)
-    for (pp, pshape, pbound) in post_wait:
-        tape.launch(pp, pshape, [0] * len(pshape), pbound)
-    # staging buffers are torch allocations consumed on the launching stream: the caching allocator reuses them in
-    # stream order, so no host synchronisation is needed here (the tape keeps the references until the next flush)
-    _done()
-
-
-def _remap_iota(prog, order):
-    """Iteration dims were permuted to `order`: point IOTA operands at the new positions."""
-    if not prog.uses_iota:
-        return prog
-    memo = prog.__dict__.setdefault("_remapped", {})
-    hit = memo.get(tuple(order))
-    if hit is not None:
-        return hit  # (one object per permutation: it keys the launch memo)
-    import copy
-
-    p = copy.copy(prog)
-    p.__dict__.pop("_remapped", None)
-    p.__dict__.pop("_packed", None)
-    inv = {d: i for i, d in enumerate(order)}
-    p.insns = []
-    for f in prog.insns:
-        g = dict(f)
-        for nm in ("a", "b", "c"):
-            if g[nm + "_kind"] == cabi.K_IOTA:
-                g[nm + "_idx"] = inv[g[nm + "_idx"]]
-        p.insns.append(g)
-    p.uses_iota = {inv[d] for d in prog.uses_iota}
-    memo[tuple(order)] = p
-    return p
-
-
-# =============================================================================================
 # ndarray
 # =============================================================================================
 def unify_args(lhs, rhs, dtype):
@@ -2122,9 +1548,6 @@ def _np_reduce(op):
     return {"sum": np.sum, "prod": np.prod, "min": np.min, "max": np.max, "all": np.all, "any": np.any}[op]
 
 
-_ALLREDUCE_OP = {"sum": "SUM", "prod": "PRODUCT", "min": "MIN", "max": "MAX", "all": "MIN", "any": "MAX"}
-
-
 def _host_identity(op, dtype):
     dtype = np.dtype(dtype)
     if op in ("sum", "any"):
@@ -2138,8 +1561,6 @@ def _host_identity(op, dtype):
 def _local_partial_tensor(red_arr, n, op):
     """This rank's block of the partial array as a flat device tensor of n elements in the accumulator dtype (float64 /
     int64) - the reduction's identity when the rank holds no part."""
-    import torch
-
     w = common.worker_num
     acc_dt = torch.float64 if red_arr.dtype.kind == "f" else torch.int64
     sv = red_arr.distribution[w]
@@ -2160,13 +1581,9 @@ def _reduction2b(red_arr, op, dtype, asarray):
         sl = (0,) * red_arr.ndim if not asarray else (slice(0, 1),) + (0,) * (red_arr.ndim - 1)
         return red_arr[sl]
     if common.num_workers > 1:
-        import torch.distributed as dist
-
         DAG.instantiate(red_arr)
-        RT.ensure_process_group()
         t = _local_partial_tensor(red_arr, 1, op)
-        dist.all_reduce(t, op=getattr(dist.ReduceOp, _ALLREDUCE_OP[op]))
-        RT.collectives += 1
+        RT.all_reduce(t, op)
         val = t.cpu().numpy()[0]
         if op in ("all", "any"):
             val = np.bool_(val != 0)
@@ -2207,17 +1624,11 @@ def _reduction2(red_arr, op, redop, dtype, axis, keepdims):
     if builtins.all(x == 1 for x in k):
         return red_arr if keepdims else red_arr[sl1]
     kept_elems = int(np.prod([red_arr.shape[d] for d in range(nd) if d not in axis]))
-    if common.num_workers > 1 and op in _ALLREDUCE_OP and kept_elems <= (1 << 24) and _split_only_along(red_arr, axis):
-        import torch
-        import torch.distributed as dist
-
+    if common.num_workers > 1 and op in ALLREDUCE_OP and kept_elems <= (1 << 24) and _split_only_along(red_arr, axis):
         DAG.instantiate(red_arr)
-        RT.ensure_process_group()
         w = common.worker_num
         t = _local_partial_tensor(red_arr, kept_elems, op)
-        dist.all_reduce(t, op=getattr(dist.ReduceOp, _ALLREDUCE_OP[op]))
-        RT.collectives += 1
-        RT.bytes_sent += kept_elems * t.element_size()
+        RT.all_reduce(t, op)
         out_shape = tuple(1 if d in axis else red_arr.shape[d] for d in range(nd))
         arr = ndarray(out_shape, dtype=red_arr.dtype, flex_dist=False)
         sh = RT.create_array(arr.gid, _local_shape(arr.bdarray.distribution, w), arr.dtype, arr.bdarray.pad)
@@ -2376,8 +1787,6 @@ def _is_whole_shard(sv, sh):
 
 def _part_to_host(nd, w, out=None, non_blocking=False):
     """This worker's part of view `nd` as a contiguous host array (get_view, ramba/ramba.py:2160-2176)."""
-    import torch
-
     if nd.bdarray.failed is not None:
         _raise_failed(nd.bdarray)
     sv = nd.distribution[w]
@@ -2415,8 +1824,6 @@ def _part_to_host(nd, w, out=None, non_blocking=False):
 
 def gather_to_host(nd, out=None, non_blocking=False):
     """Full NumPy copy of a distributed view on every rank (asarray, ramba/ramba.py:5735-5765)."""
-    import torch
-
     w, W = common.worker_num, common.num_workers
     if W == 1:
         sv = nd.distribution[0]
@@ -2430,9 +1837,6 @@ def gather_to_host(nd, out=None, non_blocking=False):
         return ret
     ret = np.empty(nd.shape, dtype=nd.dtype) if out is None else out
     mine = _part_to_host(nd, w)
-    RT.ensure_process_group()
-    import torch.distributed as dist
-
     store_dt = np.dtype(np.uint8) if nd.dtype == np.bool_ else nd.dtype
     for i in range(W):
         sv = nd.distribution[i]
@@ -2447,7 +1851,7 @@ def gather_to_host(nd, out=None, non_blocking=False):
         else:
             t = torch.empty(nbytes, dtype=torch.uint8)
         t = t.to(RT.device)
-        dist.broadcast(t, src=i)
+        RT.broadcast(t, i)
         part = t.cpu().numpy().view(store_dt).reshape(shape)
         if nd.dtype == np.bool_:
             part = part.astype(np.bool_)
@@ -2464,8 +1868,6 @@ def getitem_global(nd, index):
 
 def fromarray(x, local_border=0, dtype=None, **kwargs):
     """Distribute a NumPy array: every rank uploads its own block (ramba/ramba.py:8785-8850)."""
-    import torch
-
     if isinstance(x, numbers.Number):
         return array(x)
     x = np.asarray(x)
@@ -2500,8 +1902,6 @@ def fromarray_local(block, shape, dtype=None, **kwargs):
     """SPMD extension (no reference counterpart): every rank supplies ITS OWN block of a global
     array of shape `shape` (block shape = this rank's division under the default distribution).
     Used when the global array never exists on one host (bench.py's multi-GPU e2e leg)."""
-    import torch
-
     block = np.asarray(block)
     if dtype is None:
         dtype = block.dtype
@@ -2916,8 +2316,6 @@ def reshape_copy(arr, newshape):
     runs of consecutive linear indices, every (source rank, destination rank) pair exchanges the intersections of its runs
     - packed into one buffer per peer, one grouped send / receive - and runs of equal length at constant steps are single
     2-D strided copies on the GPU (ramba_b200/redistribute.py)."""
-    import torch
-
     from . import redistribute as R
 
     arr = _as_nd(arr)
@@ -2968,10 +2366,7 @@ def reshape_copy(arr, newshape):
         copy_groups(pl, my_sloc[ia] + (ps - my_s[ia]), my_dloc[ib] + (ps - my_d[ib]), sh_src.ptr(0), sh_dst.ptr(0), sh_src.bounds, sh_dst.bounds)
     if W == 1:
         return out
-    RT.ensure_process_group()
-    import torch.distributed as dist
-
-    ops, bufs, unpack = [], [], []
+    ops, unpack = [], []
     tdt = torch_dtype(arr.dtype)
     for peer in range(W):
         if peer == w:
@@ -2983,24 +2378,20 @@ def reshape_copy(arr, newshape):
             n = int(pl.sum())
             buf = torch.empty(n, dtype=tdt, device=RT.device)
             copy_groups(pl, my_sloc[ia] + (ps - my_s[ia]), np.cumsum(pl) - pl, sh_src.ptr(0), buf.data_ptr(), sh_src.bounds, None)
-            ops.append(dist.P2POp(dist.isend, buf.view(torch.uint8), peer))
-            bufs.append(buf)
-            RT.bytes_sent += n * isz
+            ops.append((True, buf, peer))
         # what I need from `peer`'s source block
         p_s, p_sl, _ = runs(src.shape, sdist, peer, None)
         ia, ib, ps, pl = R.intersect_runs(p_s, p_sl, my_d, my_dl)
         if len(ps):
             n = int(pl.sum())
             buf = torch.empty(n, dtype=tdt, device=RT.device)
-            ops.append(dist.P2POp(dist.irecv, buf.view(torch.uint8), peer))
-            bufs.append(buf)
+            ops.append((False, buf, peer))
             unpack.append((pl, np.cumsum(pl) - pl, my_dloc[ib] + (ps - my_d[ib]), buf))
-    if ops:
-        for wk in dist.batch_isend_irecv(ops):
-            wk.wait()  # (the launching stream waits; the host does not)
+    for wk in RT.p2p(ops):
+        wk.wait()  # (the launching stream waits; the host does not)
     for (pl, so, do, buf) in unpack:
         copy_groups(pl, so, do, buf.data_ptr(), sh_dst.ptr(0), None, sh_dst.bounds)
-    RT.keepalive = bufs
+    RT.keepalive = [b for (_, b, _) in ops]
     return out
 
 
@@ -3448,8 +2839,6 @@ def _scan_native(a, axis, op, dtype):
     rank scans its own block; when the array is cut along the scan axis the block totals are all-gathered and every rank
     folds the totals of the blocks before its own into its part (the reference passes boundary values worker to worker,
     ramba/ramba.py:3378-3437).  Returns None when this layout / dtype is not covered (caller falls back)."""
-    import torch
-
     out_dtype = np.dtype(dtype) if dtype is not None else a.dtype
     if out_dtype.kind in "iub" and out_dtype.itemsize < 8:
         out_dtype = np.dtype(np.int64)  # NumPy: small integers accumulate in the platform integer
@@ -3491,13 +2880,8 @@ def _scan_native(a, axis, op, dtype):
     if not mine_empty:
         RT.cumulative(sh_src.ptr(0), sh_res.ptr(0), code, n_outer, length, n_inner, op, None, totals.data_ptr() if totals is not None else None)
     if split_axis and W > 1:
-        import torch.distributed as tdist
-
-        RT.ensure_process_group()
         allt = torch.empty(W * ncols, dtype=acc_dt, device=RT.device)
-        tdist.all_gather_into_tensor(allt, totals)
-        RT.collectives += 1
-        RT.bytes_sent += ncols * 8 * (W - 1)
+        RT.all_gather(allt, totals).wait()
         if not mine_empty:
             before = [p for p in range(W) if not shardview.is_empty(dist[p]) and int(dist[p].start[axis]) < int(dist[w].start[axis])]
             if before:

@@ -19,11 +19,13 @@ import numbers
 import os
 
 import numpy as np
+import torch
 
 from . import _cabi as cabi
 from . import common
 from . import ramba as _r
 from .program import E, Iota
+from .runtime import RT
 
 _M64 = (1 << 64) - 1
 
@@ -54,15 +56,8 @@ def _fresh_seed():
     """A seed from os.urandom on rank 0, broadcast so that every SPMD rank draws the same arrays."""
     seed = int.from_bytes(os.urandom(8), "little")
     if common.num_workers > 1:
-        import torch
-        import torch.distributed as dist
-
-        from .runtime import RT
-
-        RT.ensure_process_group()
         t = torch.tensor([seed - (1 << 64) if seed >= (1 << 63) else seed], dtype=torch.int64).to(RT.device)
-        dist.broadcast(t, src=0)
-        RT.collectives += 1
+        RT.broadcast(t, 0)
         seed = int(t.cpu().item()) & _M64
     return seed
 

@@ -7,12 +7,9 @@ every rank runs the driver and calls its own runtime directly.
   * shards: one flat torch tensor per (gid) holding this worker's block, allocated lazily at the
     first flush that touches it (ramba/ramba.py:3506-3523, 1947-2005) and freed when the last
     handle dies (destroy_array, ramba/ramba.py:1943-1945);
-  * run_deferred_ops: classifies every operand view as local / partly remote (is_compat /
-    get_overlaps / intersect, ramba/ramba.py:3558-3644), exchanges the pieces that cross GPUs
-    with grouped NCCL send/recv instead of pickled mailbox messages (ramba/ramba.py:3646-3693),
-    cuts the iteration box into ranges in which every operand has exactly one source
-    (get_range_splits_list, ramba/ramba.py:3698-3706) and launches the op list once per range
-    through the C-ABI (ramba/ramba.py:3758-3780).
+  * launch: binds an op list to one range and calls the C-ABI (ramba/ramba.py:3758-3780);
+  * transfers: grouped NCCL send / receive, all-gather, all-reduce and broadcast instead of pickled
+    mailbox messages (ramba/ramba.py:3646-3693), each counted in bytes_sent / collectives by one rule.
 
 PyTorch is used for device memory, streams and torch.distributed only.
 """
@@ -21,6 +18,7 @@ import os
 
 import numpy as np
 import torch
+import torch.distributed as dist
 
 from . import _cabi as cabi
 from . import common
@@ -43,6 +41,10 @@ _TORCH_DTYPE = {
 
 def torch_dtype(dt):
     return _TORCH_DTYPE[np.dtype(dt)]
+
+
+# reductions an all-reduce can combine, and how (all / any of 0/1 values are min / max)
+ALLREDUCE_OP = {"sum": "SUM", "prod": "PRODUCT", "min": "MIN", "max": "MAX", "all": "MIN", "any": "MAX"}
 
 
 class Shard:
@@ -143,8 +145,6 @@ class CudaBackend:
         return scratch
 
     def init_process_group(self):
-        import torch.distributed as dist
-
         dist.init_process_group("nccl", device_id=self.device)
 
     def synchronize(self):
@@ -162,7 +162,7 @@ class Runtime:
         self._pg_ready = False
         self.launches = 0
         self.bytes_sent = 0
-        self.collectives = 0  # all-gather / all-reduce calls issued
+        self.collectives = 0  # all-gather / all-reduce / broadcast calls issued
         self.ring_receives = 0  # halo pieces received into the ring of a padded block (getborder)
         self.keepalive = None  # staging buffers of the last flush
         self.profile_events = None  # list -> (start, end, n_insns) CUDA events around every launch
@@ -204,11 +204,47 @@ class Runtime:
     def ensure_process_group(self):
         if common.num_workers <= 1 or self._pg_ready:
             return
-        import torch.distributed as dist
-
         if not dist.is_initialized():
             self.be().init_process_group()
         self._pg_ready = True
+
+    # ---- transfers between ranks: the only code of the package that talks to other ranks.  Counting rule (DESIGN.md §4):
+    # a grouped send / receive adds the bytes of every send; an all-gather adds one collective and the bytes of this rank's
+    # part times W-1; an all-reduce one collective and the bytes of the tensor; a broadcast one collective and, on the
+    # source rank, the bytes of the tensor times W-1.
+    def p2p(self, ops):
+        """ops: [(is_send, tensor, peer)] -> the works of ONE grouped send / receive of their bytes, not waited for."""
+        if not ops:
+            return []
+        self.ensure_process_group()
+        pending = []
+        for is_send, t, peer in ops:
+            if is_send:
+                self.bytes_sent += t.numel() * t.element_size()
+            pending.append(dist.P2POp(dist.isend if is_send else dist.irecv, t.view(torch.uint8), peer))
+        return dist.batch_isend_irecv(pending)
+
+    def all_gather(self, full, mine):
+        """Every rank's `mine`, in rank order, into `full`; returns the work, not waited for."""
+        self.ensure_process_group()
+        self.collectives += 1
+        self.bytes_sent += mine.numel() * mine.element_size() * (common.num_workers - 1)
+        return dist.all_gather_into_tensor(full.view(torch.uint8), mine.view(torch.uint8), async_op=True)
+
+    def all_reduce(self, t, op):
+        """t = op over every rank's t, in place; op: sum prod min max all any."""
+        self.ensure_process_group()
+        self.collectives += 1
+        self.bytes_sent += t.numel() * t.element_size()
+        dist.all_reduce(t, op=getattr(dist.ReduceOp, ALLREDUCE_OP[op]))
+
+    def broadcast(self, t, src):
+        """Rank src's t into every rank's t, in place."""
+        self.ensure_process_group()
+        self.collectives += 1
+        if common.worker_num == src:
+            self.bytes_sent += t.numel() * t.element_size() * (common.num_workers - 1)
+        dist.broadcast(t, src=src)
 
     # ---- shard storage --------------------------------------------------------------------
     def create_array(self, gid, local_shape, dtype, border=0):
@@ -435,7 +471,7 @@ def fill_template(template, views, red_outs=None, red_scratch=None):
 
 
 _launch_cache = {}
-# RB200_VERIFY_PLAN_CACHE=1: every hit of the launch memo (here) and of the flush memo (ramba.run_deferred_ops) is
+# RB200_VERIFY_PLAN_CACHE=1: every hit of the launch memo (here) and of the flush memo (flush.run_deferred_ops) is
 # checked against planning the same thing again
 _VERIFY_PLAN_CACHE = bool(int(os.environ.get("RB200_VERIFY_PLAN_CACHE", "0")))
 

@@ -100,6 +100,11 @@ def main():
     rb.sync()
     if common.worker_num == 0:
         onp.savez(sys.argv[1], **res)
+    if common.num_workers > 1:  # leave the process group cleanly before the interpreter exits
+        import torch.distributed as dist
+
+        dist.barrier()
+        dist.destroy_process_group()
     print("ok rank=%d launches=%d" % (common.worker_num, RT.launches))
 
 

@@ -129,15 +129,15 @@ def test_dtypes_are_part_of_the_key(verified_memo):
         assert got.dtype == exp.dtype and onp.array_equal(got, exp)
 
 
-# ---- the flush memo (ramba.py::run_deferred_ops): every flush is recorded as a script, later flushes with the same key
+# ---- the flush memo (flush.py::run_deferred_ops): every flush is recorded as a script, later flushes with the same key
 # replay it
 @pytest.fixture
 def verified_plans(oracle_engine, monkeypatch):
-    from ramba_b200 import ramba
+    from ramba_b200 import flush
 
-    monkeypatch.setattr(ramba, "_VERIFY_PLAN_CACHE", True)
-    ramba._plan_cache.clear()
-    return ramba
+    monkeypatch.setattr(flush, "_VERIFY_PLAN_CACHE", True)
+    flush._plan_cache.clear()
+    return flush
 
 
 def test_repeated_flush_is_replayed_from_its_script(verified_plans, monkeypatch):

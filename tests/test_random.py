@@ -212,14 +212,14 @@ def _fused_and_kept(rb):
 @pytest.mark.parametrize("mode", ["default", "no_dag", "verify_lower", "verify_plan"])
 def test_fused_and_materialised_draws_agree(engine, monkeypatch, mode):
     import ramba_b200 as rb
-    from ramba_b200 import ramba, runtime
+    from ramba_b200 import flush, ramba, runtime
 
     if mode == "no_dag":
         monkeypatch.setattr(ramba, "NO_DAG", True)
     elif mode == "verify_lower":
         monkeypatch.setattr(ramba, "_VERIFY_LOWER_CACHE", True)
     elif mode == "verify_plan":
-        monkeypatch.setattr(ramba, "_VERIFY_PLAN_CACHE", True)
+        monkeypatch.setattr(flush, "_VERIFY_PLAN_CACHE", True)
         monkeypatch.setattr(runtime, "_VERIFY_PLAN_CACHE", True)
     for _ in range(2):  # the second round hits the memos
         xs, kept, folded, s_fold = _fused_and_kept(rb)
