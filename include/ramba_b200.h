@@ -40,7 +40,7 @@
 extern "C" {
 #endif
 
-#define RB200_ABI_VERSION 6
+#define RB200_ABI_VERSION 7
 
 #define RB200_MAX_DIMS 5     /* iteration dims after host-side collapsing            */
 #define RB200_MAX_VIEWS 16   /* distinct array views per fused op                    */
@@ -322,6 +322,48 @@ typedef struct rb200_route_table {
 int64_t rb200_route_scratch_bytes(int64_t n, int32_t n_ranks);
 int rb200_route(const rb200_route_table* table, const int64_t* lin, int64_t n, int64_t* offsets, int64_t* slots, int64_t* counts,
                 uint64_t* bad, void* scratch, void* stream);
+
+/* ---- grouped reduction along one axis (groupby) -----------------------------------------------------------------------
+ * What it stands for in the reference: RambaGroupby's aggregations (ramba/ramba.py:10185-10643), sreduce_index over Python
+ * callables.  The host turns the labels of the grouped axis into a CSR table once; one launch reads every source element
+ * once and writes every output once.
+ *   SUM, PROD, MIN, MAX: as the engine's reductions (MIN / MAX: `b < a ? b : a`, so a NaN member is skipped);
+ *   NANSUM: the sum of the members that are not NaN; NANCOUNT: their number;
+ *   SQDEV: sum((x - center[o, g, i])**2), the difference and the square rounded separately.
+ * Accumulator class of `out`: F64 for float sources and for SQDEV, I64 (wrapping) for integer sources otherwise.  An empty
+ * group gets the identity: 0, 1, the largest / smallest value of the class (+-inf for F64), 0, 0, 0.
+ * Fold order: the axis is cut into chunks of C consecutive positions (rb200_describe_group_plan states C, a function of the
+ * view's shape and G only); the members of a group inside a chunk are combined in ascending order starting from the
+ * identity, and the chunk partials in chunk order, again starting from the identity.  No atomics.                     */
+enum rb200_group_op {
+  RB200_GROUP_SUM = 0,
+  RB200_GROUP_PROD = 1,
+  RB200_GROUP_MIN = 2,
+  RB200_GROUP_MAX = 3,
+  RB200_GROUP_NANSUM = 4,
+  RB200_GROUP_NANCOUNT = 5,
+  RB200_GROUP_SQDEV = 6,
+  RB200_GROUP_NUM_OPS = 7
+};
+
+typedef struct rb200_group_table {
+  int32_t n_groups;        /* G >= 1                                                                              */
+  int64_t len;             /* extent of the grouped axis in this view                                             */
+  const int64_t* offsets;  /* device, G+1 entries: offsets[0] = 0, ascending, offsets[G] = len                    */
+  const int64_t* members;  /* device, len entries: positions along the axis, grouped by label and ascending inside
+                              each group (a permutation of 0..len-1)                                              */
+} rb200_group_table;
+
+/* out[o, g, i] = op over t in members[offsets[g]:offsets[g+1]] of src[o, t, i] (o: the axes before `axis`, i: the axes
+ * after it).  src_dtype: RB200_F64, F32, I64 or I32 (matching src->elem_bytes).  out is contiguous in the accumulator
+ * class; center (SQDEV only): the same shape as out, F64.  scratch: rb200_group_reduce_scratch_bytes() bytes (may be NULL
+ * when that is 0).  Malformed arguments are rejected with a reason before any device query.                          */
+int rb200_group_reduce(const rb200_index_view* src, int32_t src_dtype, int32_t axis, const rb200_group_table* groups, int32_t op,
+                       const void* center, void* out, void* scratch, void* stream);
+int64_t rb200_group_reduce_scratch_bytes(const rb200_index_view* src, int32_t axis, int32_t n_groups);
+/* One text line: form (row / column / general), chunk C, chunks, CTAs, scratch.  Needs no device.  NULL on a malformed
+ * argument (reason in rb200_last_error); the text stays valid until the next call on this thread.                    */
+const char* rb200_describe_group_plan(const rb200_index_view* src, int32_t axis, int32_t n_groups);
 
 /* Which kernel rb200_run_deferred_ops would run `op` on and how (staged views, halos, TMA or cp.async loader, ring depth,
  * lean instructions, CTAs), as one text line in out[0..cap).  Needs no device and touches no pointer: the counterpart

@@ -10,7 +10,7 @@ raises.
 import ctypes as C
 import os
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 MAX_DIMS = 5
 MAX_VIEWS = 16
 MAX_SCALARS = 32
@@ -37,6 +37,8 @@ OP = {name: i for i, name in enumerate(OPS)}
 RED_ADD, RED_MUL, RED_MIN, RED_MAX = range(4)
 # output forms of PHILOX (imm)
 PHILOX_UNIFORM64, PHILOX_UNIFORM32, PHILOX_NORMAL64, PHILOX_INTEGER = range(4)
+# grouped-reduction ops (rb200_group_reduce)
+GROUP_SUM, GROUP_PROD, GROUP_MIN, GROUP_MAX, GROUP_NANSUM, GROUP_NANCOUNT, GROUP_SQDEV = range(7)
 
 
 class Insn(C.Structure):
@@ -112,6 +114,15 @@ class RouteTable(C.Structure):
     ]
 
 
+class GroupTable(C.Structure):
+    _fields_ = [
+        ("n_groups", C.c_int32),
+        ("len", C.c_int64),
+        ("offsets", C.c_void_p),
+        ("members", C.c_void_p),
+    ]
+
+
 assert C.sizeof(Insn) == 16
 
 # every symbol include/ramba_b200.h declares
@@ -131,6 +142,9 @@ EXPORTS = [
     "rb200_scatter",
     "rb200_route",
     "rb200_route_scratch_bytes",
+    "rb200_group_reduce",
+    "rb200_group_reduce_scratch_bytes",
+    "rb200_describe_group_plan",
 ]
 
 _LIB = None
@@ -189,6 +203,13 @@ def load():
     lib.rb200_route.restype = C.c_int
     lib.rb200_route_scratch_bytes.argtypes = [C.c_int64, C.c_int32]
     lib.rb200_route_scratch_bytes.restype = C.c_int64
+    lib.rb200_group_reduce.argtypes = [C.POINTER(IndexView), C.c_int32, C.c_int32, C.POINTER(GroupTable), C.c_int32, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p]
+    lib.rb200_group_reduce.restype = C.c_int
+    lib.rb200_group_reduce_scratch_bytes.argtypes = [C.POINTER(IndexView), C.c_int32, C.c_int32]
+    lib.rb200_group_reduce_scratch_bytes.restype = C.c_int64
+    lib.rb200_describe_group_plan.argtypes = [C.POINTER(IndexView), C.c_int32, C.c_int32]
+    lib.rb200_describe_group_plan.restype = C.c_char_p
     if lib.rb200_abi_version() != ABI_VERSION:
         raise CabiError("libramba_b200.so ABI %d != binding ABI %d: rebuild" % (lib.rb200_abi_version(), ABI_VERSION))
     _LIB = lib
@@ -299,3 +320,39 @@ def route(table, lin, n, offsets, slots, counts, bad, scratch, stream=None):
 
 def route_scratch_bytes(n, n_ranks):
     return int(load().rb200_route_scratch_bytes(n, n_ranks))
+
+
+def group_table(n_groups, length, offsets, members):
+    """A GroupTable struct over device (or, for the restatement, host) addresses of offsets and members."""
+    t = GroupTable()
+    t.n_groups, t.len, t.offsets, t.members = int(n_groups), int(length), offsets, members
+    return t
+
+
+def group_reduce(view, src_dtype, axis, table, op, center, out, scratch, stream=None):
+    check(load().rb200_group_reduce(C.byref(view), src_dtype, axis, C.byref(table), op, _p(center), _p(out), _p(scratch), _p(stream)))
+
+
+def group_reduce_scratch_bytes(view, axis, n_groups):
+    n = int(load().rb200_group_reduce_scratch_bytes(C.byref(view), axis, n_groups))
+    if n < 0:
+        check(1)
+    return n
+
+
+def describe_group_plan(view, axis, n_groups):
+    """One text line: the form, the chunk C and the split the library would reduce this view with (no device needed)."""
+    lib = load()
+    s = lib.rb200_describe_group_plan(C.byref(view), axis, n_groups)
+    if s is None:
+        check(1)
+    return s.decode()
+
+
+def group_plan_fields(text):
+    """{key: value} of a rb200_describe_group_plan line (integers where they parse)."""
+    out = {}
+    for kv in text.split():
+        k, v = kv.split("=", 1)
+        out[k] = int(v) if v.lstrip("-").isdigit() else v
+    return out

@@ -9,6 +9,7 @@
 
 #include "rb200_launch.h"
 #include "rb200_handlers.h"
+#include "rb200_group.h"
 #include "rb200_index.h"
 #include "rb200_rng.h"
 #include "rb200_stream.h"
@@ -673,6 +674,18 @@ static int check_route_table(const rb200_route_table* t, RouteParams* R) {
   return 0;
 }
 
+// ---- grouped reduction: argument checks (before any device query) and the plan
+static int check_group_args(const rb200_index_view* src, int axis, int n_groups, GroupPlan* P) {
+  if (const int rc = check_index_view(src, "group_reduce")) return rc;
+  if (axis < 0 || axis >= src->ndim) return fail("group_reduce: axis out of range");
+  if (n_groups < 1) return fail("group_reduce: n_groups must be >= 1");
+  make_group_plan(*src, axis, n_groups, P);
+  if (P->ctas >= (1ll << 31)) return fail("group_reduce: too many outputs for one launch");
+  return 0;
+}
+
+static thread_local std::string g_group_plan_text;
+
 extern "C" {
 
 const char* rb200_last_error(void) { return g_last_error.c_str(); }
@@ -771,6 +784,46 @@ int rb200_route(const rb200_route_table* table, const int64_t* lin, int64_t n, i
   const cudaError_t e = launch_route(R, (const long long*)lin, n, (long long*)offsets, (long long*)slots, (long long*)counts,
                                      (unsigned long long*)bad, scratch, sms, (cudaStream_t)stream_v);
   if (e != cudaSuccess) return fail_cuda("route kernel launch", e);
+  g_launches.fetch_add(1);
+  return 0;
+}
+
+int64_t rb200_group_reduce_scratch_bytes(const rb200_index_view* src, int32_t axis, int32_t n_groups) {
+  GroupPlan P;
+  if (check_group_args(src, axis, n_groups, &P)) return -1;
+  return (int64_t)P.scratch_bytes;
+}
+
+const char* rb200_describe_group_plan(const rb200_index_view* src, int32_t axis, int32_t n_groups) {
+  GroupPlan P;
+  if (check_group_args(src, axis, n_groups, &P)) return nullptr;
+  char buf[240];
+  snprintf(buf, sizeof(buf), "kernel=group form=%s chunk=%lld chunks=%d cta_chunks=%d ctas_per_row=%d kept=%lld groups=%d ctas=%lld scratch=%lld",
+           group_form_name(P.form), P.C, P.S, P.ncl, P.K, P.nkept, P.G, P.ctas, P.scratch_bytes);
+  g_group_plan_text = buf;
+  return g_group_plan_text.c_str();
+}
+
+int rb200_group_reduce(const rb200_index_view* src, int32_t src_dtype, int32_t axis, const rb200_group_table* groups, int32_t op, const void* center,
+                       void* out, void* scratch, void* stream_v) {
+  if (op < 0 || op >= RB200_GROUP_NUM_OPS) return fail("group_reduce: bad op");
+  if (src_dtype != RB200_F64 && src_dtype != RB200_F32 && src_dtype != RB200_I64 && src_dtype != RB200_I32)
+    return fail("group_reduce: source dtype must be float64, float32, int64 or int32");
+  if (src && dtype_size(src_dtype) != src->elem_bytes) return fail("group_reduce: elem_bytes does not match the source dtype");
+  if (!groups) return fail("group_reduce: null group table");
+  GroupPlan P;
+  if (const int rc = check_group_args(src, axis, groups->n_groups, &P)) return rc;
+  if (groups->len != src->shape[axis]) return fail("group_reduce: table len differs from the extent of the grouped axis");
+  if (!groups->offsets || (groups->len > 0 && !groups->members)) return fail("group_reduce: null table array");
+  if (op == RB200_GROUP_SQDEV && !center) return fail("group_reduce: SQDEV needs center");
+  if (!out) return fail("group_reduce: null out");
+  if (P.scratch_bytes && !scratch) return fail("group_reduce: null scratch (this plan splits the axis)");
+  if (P.nkept == 0) return 0;
+  const int sms = sm_count();
+  if (sms <= 0) return fail("no usable CUDA device (libramba_b200 has no CPU path)");
+  const cudaError_t e = launch_group(P, src_dtype, op, (const long long*)groups->offsets, (const long long*)groups->members, (const double*)center, out,
+                                     scratch, (cudaStream_t)stream_v);
+  if (e != cudaSuccess) return fail_cuda("group kernel launch", e);
   g_launches.fetch_add(1);
   return 0;
 }

@@ -1692,6 +1692,21 @@ array_inplace_binop_funcs = {
 }
 for _n, _t in array_inplace_binop_funcs.items():
     setattr(ndarray, _n, _make_binop(_n, _t, inplace=True))
+
+
+def _ndarray_groupby(self, dim, value_to_group, num_groups=None):
+    """Group the positions of axis `dim` by the integer labels `value_to_group` (ramba/ramba.py:6896-6899): a RambaGroupby
+    whose sum / prod / min / max / count / mean / nanmean / var / std reduce every group on the grouped-reduction kernel
+    (ramba_b200/groupby.py).  num_groups=None means value_to_group.max() + 1."""
+    from .groupby import RambaGroupby
+
+    return RambaGroupby(self, dim, value_to_group, num_groups)
+
+
+ndarray.groupby = _ndarray_groupby
+from . import groupby as _groupby_module  # noqa: E402
+
+_groupby_module._install_binops(list(array_binop_funcs) + list(array_binop_rfuncs))
 ndarray.__hash__ = None
 
 

@@ -144,6 +144,13 @@ class CudaBackend:
         cabi.route(table, lin, n, offsets, slots, counts, bad, scratch.data_ptr(), self.stream_handle())
         return scratch
 
+    def group_reduce(self, view, src_code, axis, table, op, center, out):
+        """rb200_group_reduce on the current stream; returns the scratch buffer (the caller keeps it alive)."""
+        nbytes = cabi.group_reduce_scratch_bytes(view, axis, table.n_groups)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device) if nbytes else None
+        cabi.group_reduce(view, src_code, axis, table, op, center, out, scratch.data_ptr() if nbytes else None, self.stream_handle())
+        return scratch
+
     def init_process_group(self):
         dist.init_process_group("nccl", device_id=self.device)
 
@@ -444,6 +451,14 @@ class Runtime:
         """Inclusive scan of one local block through the C-ABI (rb200_cumulative)."""
         self.keepalive_scan = self.be().cumulative(src_ptr, dst_ptr, code, n_outer, length, n_inner, redop, carry_in, totals_out)
         self.launches += 1
+
+    def group_reduce(self, view, src_code, axis, table, op, center, out):
+        """Grouped reduction of one local view along `axis` through the C-ABI (rb200_group_reduce): out (device address,
+        accumulator class) receives op over the members of every group (table: a cabi.GroupTable).  Returns the scratch
+        buffer (or None); the caller holds it until the launches that follow on this stream have been enqueued."""
+        scratch = self.be().group_reduce(view, src_code, axis, table, op, center, out)
+        self.launches += 1
+        return scratch
 
     def synchronize(self):
         if self.backend is not None:
