@@ -41,11 +41,11 @@ def card():
 
 
 def kernel_time(rb, A, gb, reps):
-    from ramba_b200 import _cabi, advindex
+    from ramba_b200 import _cabi, blocks
     from ramba_b200.program import rb_dtype
     from ramba_b200.runtime import RT
 
-    view = advindex._local_view(A)
+    view = blocks.index_view(A)
     table = gb._table(0, A.shape[gb.dim])
     G = gb.num_groups
     n_out = A.size // A.shape[gb.dim] * G

@@ -23,6 +23,7 @@ import numpy as np
 import torch
 
 from . import _cabi as cabi
+from . import blocks
 from . import common
 from . import shardview
 from .flush import _local_shape
@@ -189,33 +190,6 @@ def _check_array_terms(src_shape, terms):
             _check_bounds(p.asarray(), axis, src_shape[axis])
 
 
-def _itemsize(dtype):
-    return np.dtype(np.uint8 if dtype == np.bool_ else dtype).itemsize
-
-
-def _shard(nd):
-    bd = nd.bdarray
-    sh = RT.shards.get(nd.gid) or RT.create_array(nd.gid, _local_shape(bd.distribution, common.worker_num), bd.dtype, bd.pad)
-    bd.remote_constructed = True
-    bd.flex_dist = False
-    return sh
-
-
-def _local_view(nd):
-    """IndexView of this rank's part of view nd (the whole view at one rank)."""
-    sv = nd.distribution[common.worker_num]
-    sh = _shard(nd)
-    off, st = RT.bind_view(sv, sh.strides, shardview.clean_range(sv))
-    return cabi.index_view(sh.ptr(off), [int(x) for x in sv.size], st, _itemsize(nd.dtype), sh.bounds)
-
-
-def _flat_shard_view(nd):
-    """1-D IndexView over this rank's whole shard of nd, indexed by element offsets from its interior origin."""
-    sh = _shard(nd)
-    n = sh.buf.numel() - sh.origin
-    return cabi.index_view(sh.ptr(0), [n], [1], _itemsize(nd.dtype), sh.bounds)
-
-
 def _route_table(nd):
     """The partition of view nd as a grid: every rank's box, its owner and where the owner keeps it."""
     bd = nd.bdarray
@@ -247,11 +221,6 @@ def _route_table(nd):
     return cabi.route_table(shape, cuts, owners, offsets, strides, common.num_workers)
 
 
-def _needs_copy(nd):
-    return builtins.any(int(sv.axis_map[d]) < 0 and nd.shape[d] > 1 for sv in nd.distribution if not shardview.is_empty(sv)
-                        for d in range(len(nd.shape)))
-
-
 def _exchange_counts(counts):
     """counts: this rank's requests per owner (device int64, W entries) -> M[p][q] on the host, for every p."""
     W = common.num_workers
@@ -262,15 +231,13 @@ def _exchange_counts(counts):
 
 def _route(nd, lin_ptr, n):
     """Route this rank's n requests on view nd: (offsets, slots, M, starts, keep)."""
-    be = RT.be()
     W = common.num_workers
     table, keep = _route_table(nd)
     offs = torch.empty(max(n, 1), dtype=torch.int64, device=RT.device)
     slots = torch.empty(max(n, 1), dtype=torch.int64, device=RT.device)
     counts = torch.zeros(W, dtype=torch.int64, device=RT.device)
     bad = torch.zeros(1, dtype=torch.int64, device=RT.device)
-    scratch = be.route(table, lin_ptr, n, offs.data_ptr(), slots.data_ptr(), counts.data_ptr(), bad.data_ptr())
-    RT.launches += 1
+    scratch = RT.route(table, lin_ptr, n, offs.data_ptr(), slots.data_ptr(), counts.data_ptr(), bad.data_ptr())
     M = _exchange_counts(counts)
     mine = M[common.worker_num]
     starts = np.concatenate([[0], np.cumsum(mine)[:-1]]).astype(np.int64)
@@ -279,22 +246,20 @@ def _route(nd, lin_ptr, n):
 
 def _gather(src, lin_nd, out):
     """out[i] = src[lin[i]] for this rank's block of lin / out."""
-    be = RT.be()
     w, W = common.worker_num, common.num_workers
-    lin_sh, out_sh = _shard(lin_nd), _shard(out)
+    lin_sh, out_sh = blocks.block(lin_nd), blocks.block(out)
     n = int(np.prod(lin_sh.shape)) if lin_sh.shape else 1
     if shardview.is_empty(lin_nd.distribution[w]):
         n = 0
     bad = torch.zeros(1, dtype=torch.int64, device=RT.device)
     if W == 1:
-        be.gather(_local_view(src), lin_sh.ptr(0), n, out_sh.ptr(0), bad.data_ptr())
-        RT.launches += 1
-        RT.keepalive = [bad]
+        RT.gather(blocks.index_view(src), lin_sh.ptr(0), n, out_sh.ptr(0), bad.data_ptr())
+        RT.hold(bad)
         return
-    isz = _itemsize(src.dtype)
+    isz = blocks.itemsize(src.dtype)
     offs, slots, M, starts, keep = _route(src, lin_sh.ptr(0), n)
     nv = int(M[w].sum())
-    flat = _flat_shard_view(src)
+    flat = blocks.flat_index_view(src)
     rep = torch.empty(max(nv * isz, 1), dtype=torch.uint8, device=RT.device)
     ops, reqs = [], []
     for q in range(W):
@@ -307,13 +272,11 @@ def _gather(src, lin_nd, out):
     for wk in RT.p2p(ops):
         wk.wait()
     if M[w][w]:  # this rank's own elements: straight into the reply buffer
-        be.gather(flat, offs[starts[w]:].data_ptr(), int(M[w][w]), rep[starts[w] * isz:].data_ptr(), bad.data_ptr())
-        RT.launches += 1
+        RT.gather(flat, offs[starts[w]:].data_ptr(), int(M[w][w]), rep[starts[w] * isz:].data_ptr(), bad.data_ptr())
     ops, served = [], []
     for q, req in reqs:
         r = torch.empty(req.numel() * isz, dtype=torch.uint8, device=RT.device)
-        be.gather(flat, req.data_ptr(), req.numel(), r.data_ptr(), bad.data_ptr())
-        RT.launches += 1
+        RT.gather(flat, req.data_ptr(), req.numel(), r.data_ptr(), bad.data_ptr())
         ops.append((True, r, q))
         served.append(r)
     for q in range(W):
@@ -322,32 +285,28 @@ def _gather(src, lin_nd, out):
     for wk in RT.p2p(ops):
         wk.wait()
     if n:
-        be.gather(cabi.index_view(rep.data_ptr(), [nv], [1], isz), slots.data_ptr(), n, out_sh.ptr(0), bad.data_ptr())
-        RT.launches += 1
-    RT.keepalive = keep + [rep, bad, reqs, served]
+        RT.gather(cabi.index_view(rep.data_ptr(), [nv], [1], isz), slots.data_ptr(), n, out_sh.ptr(0), bad.data_ptr())
+    RT.hold(*keep, rep, bad, reqs, served)
 
 
 def _scatter(dst, lin_nd, vals):
     """dst[lin[i]] = vals[i] for this rank's block of lin / vals."""
-    be = RT.be()
     w, W = common.worker_num, common.num_workers
-    lin_sh, val_sh = _shard(lin_nd), _shard(vals)
+    lin_sh, val_sh = blocks.block(lin_nd), blocks.block(vals)
     n = int(np.prod(lin_sh.shape)) if lin_sh.shape else 1
     if shardview.is_empty(lin_nd.distribution[w]):
         n = 0
     bad = torch.zeros(1, dtype=torch.int64, device=RT.device)
     if W == 1:
-        be.scatter(_local_view(dst), lin_sh.ptr(0), n, val_sh.ptr(0), bad.data_ptr())
-        RT.launches += 1
-        RT.keepalive = [bad]
+        RT.scatter(blocks.index_view(dst), lin_sh.ptr(0), n, val_sh.ptr(0), bad.data_ptr())
+        RT.hold(bad)
         return
-    isz = _itemsize(dst.dtype)
+    isz = blocks.itemsize(dst.dtype)
     offs, slots, M, starts, keep = _route(dst, lin_sh.ptr(0), n)
     nv = int(M[w].sum())
     packed = torch.empty(max(nv * isz, 1), dtype=torch.uint8, device=RT.device)
     if n:  # the values in slot order, grouped by owner
-        be.scatter(cabi.index_view(packed.data_ptr(), [nv], [1], isz), slots.data_ptr(), n, val_sh.ptr(0), bad.data_ptr())
-        RT.launches += 1
+        RT.scatter(cabi.index_view(packed.data_ptr(), [nv], [1], isz), slots.data_ptr(), n, val_sh.ptr(0), bad.data_ptr())
     ops, got = [], []
     for q in range(W):
         if q != w and M[w][q]:
@@ -361,14 +320,12 @@ def _scatter(dst, lin_nd, vals):
             got.append((req, v))
     for wk in RT.p2p(ops):
         wk.wait()
-    flat = _flat_shard_view(dst)
+    flat = blocks.flat_index_view(dst)
     if M[w][w]:
-        be.scatter(flat, offs[starts[w]:].data_ptr(), int(M[w][w]), packed[starts[w] * isz:].data_ptr(), bad.data_ptr())
-        RT.launches += 1
+        RT.scatter(flat, offs[starts[w]:].data_ptr(), int(M[w][w]), packed[starts[w] * isz:].data_ptr(), bad.data_ptr())
     for req, v in got:
-        be.scatter(flat, req.data_ptr(), req.numel(), v.data_ptr(), bad.data_ptr())
-        RT.launches += 1
-    RT.keepalive = keep + [packed, bad, got]
+        RT.scatter(flat, req.data_ptr(), req.numel(), v.data_ptr(), bad.data_ptr())
+    RT.hold(*keep, packed, bad, got)
 
 
 def _prepare(a, index):
@@ -396,7 +353,7 @@ def getitem(a, index):
     if size == 0:
         _check_array_terms(a.shape, terms)
         return R.empty(rshape, dtype=a.dtype)
-    src = R.copy(a) if common.num_workers > 1 and _needs_copy(a) else a
+    src = R.copy(a) if common.num_workers > 1 and blocks.overlaps_across_ranks(a) else a
     lin = _address_stream(src, terms, rshape, bpos, bshape)
     out = R.create_array_with_divisions(rshape, lin.distribution, dtype=a.dtype)
     R.DAG.instantiate(src)  # pending writes of the source
@@ -417,12 +374,5 @@ def setitem(a, index, value):
     vals = R.create_array_with_divisions(rshape, lin.distribution, dtype=a.dtype)
     vals[...] = value
     R.DAG.instantiate(vals)
-    # every pending statement that reads or writes a's storage runs before the store (WAR and WAW)
-    g = a.gid
-    nodes = list(R.DAG.readers.get(g, ()))
-    if g in R.DAG.last_writer:
-        nodes.append(R.DAG.last_writer[g])
-    if nodes:
-        R.DAG._run(nodes)
-    R.deferred_op.do_ops()
+    R.DAG.before_write(a)
     _scatter(a, lin, vals)

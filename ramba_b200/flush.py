@@ -57,11 +57,12 @@ def _local_shape(bd_dist, w):
     return tuple(int(x) for x in sv.size)
 
 
-def _contig_strides(shape, bcast):
+def _contig_strides(shape, bcast=None):
+    """(C-order element strides of `shape`, 0 along the dims where bcast is true; element count)."""
     st = [0] * len(shape)
     acc = 1
     for d in reversed(range(len(shape))):
-        if bcast[d]:
+        if bcast is not None and bcast[d]:
             st[d] = 0
         else:
             st[d] = acc
@@ -230,11 +231,11 @@ class _FlushTape:
 
     def reduce_partials(self, out_ptr, in_ptr, n, k, stride_k, code, rop):
         self.actions.append(("fold", self._resolve(out_ptr), self._resolve(in_ptr), int(n), int(k), int(stride_k), int(code), int(rop)))
-        RT._reduce_partials(out_ptr, in_ptr, n, k, stride_k, code, rop, RT.stream_handle())
+        RT.reduce_partials(out_ptr, in_ptr, n, k, stride_k, code, rop)
 
     def finish(self):
         RT.ring_receives += self.ring_receives
-        RT.keepalive = self.buffers  # consumed on the launching stream; kept until the next flush
+        RT.hold(*self.buffers)  # consumed on the launching stream
         return (tuple(self.actions), self.ring_receives)
 
 
@@ -274,11 +275,11 @@ def _replay_tape(script, shards):
         elif k == "allgather":
             works.append(RT.all_gather(bufs[a[1]], bufs[a[2]]))
         else:  # fold
-            RT._reduce_partials(_addr(a[1], shards, bufs), _addr(a[2], shards, bufs), a[3], a[4], a[5], a[6], a[7], RT.stream_handle())
+            RT.reduce_partials(_addr(a[1], shards, bufs), _addr(a[2], shards, bufs), a[3], a[4], a[5], a[6], a[7])
     for wk in works:
         wk.wait()
     RT.ring_receives += ring_receives
-    RT.keepalive = bufs
+    RT.hold(*bufs)
 
 
 def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
@@ -540,7 +541,7 @@ def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
     for (pp, pshape, pbound) in post_wait:
         tape.launch(pp, pshape, [0] * len(pshape), pbound)
     # staging buffers are torch allocations consumed on the launching stream: the caching allocator reuses them in
-    # stream order, so no host synchronisation is needed here (the tape keeps the references until the next flush)
+    # stream order, so no host synchronisation is needed here (the tape holds them until the next hold)
     _done()
 
 

@@ -22,34 +22,16 @@ import numpy as np
 import torch
 
 from . import _cabi as cabi
-from . import advindex
+from . import blocks
 from . import common
 from . import shardview
-from .flush import _pack_program
-from .program import E, Lowering, np_dtype, rb_dtype
+from .flush import _contig_strides, _pack_program
+from .program import E, Lowering, np_dtype, rb_dtype, red_identity
 from .runtime import RT
 
 _KERNEL_DTYPES = tuple(np.dtype(d) for d in (np.float64, np.float32, np.int64, np.int32))
 _ALLREDUCE = {cabi.GROUP_SUM: "sum", cabi.GROUP_PROD: "prod", cabi.GROUP_MIN: "min", cabi.GROUP_MAX: "max",
               cabi.GROUP_NANSUM: "sum", cabi.GROUP_NANCOUNT: "sum", cabi.GROUP_SQDEV: "sum"}
-
-
-def _identity(op, is_float):
-    if op == cabi.GROUP_PROD:
-        return 1
-    if op == cabi.GROUP_MIN:
-        return np.inf if is_float else np.iinfo(np.int64).max
-    if op == cabi.GROUP_MAX:
-        return -np.inf if is_float else np.iinfo(np.int64).min
-    return 0
-
-
-def _c_strides(shape):
-    st, acc = [], 1
-    for s in reversed(shape):
-        st.append(acc)
-        acc *= int(s)
-    return list(reversed(st))
 
 
 def _int_bounds(dt):
@@ -175,7 +157,7 @@ class RambaGroupby:
         a = self.array_to_group
         if a.dtype not in _KERNEL_DTYPES:  # bool and small integers: one fused widening copy
             a = a.astype(np.float64 if a.dtype.kind == "f" else np.int64)
-        if common.num_workers > 1 and advindex._needs_copy(a):  # broadcast views overlap between ranks
+        if common.num_workers > 1 and blocks.overlaps_across_ranks(a):  # broadcast views overlap between ranks
             a = R.copy(a)
         R.DAG.instantiate(a)
         return a
@@ -198,6 +180,7 @@ class RambaGroupby:
         is_f = src.dtype.kind == "f" or op == cabi.GROUP_SQDEV
         tdt = torch.float64 if is_f else torch.int64
         code = cabi.F64 if is_f else cabi.I64
+        ident = red_identity(_ALLREDUCE[op], np.float64 if is_f else np.int64)
         bstart, bsize = self._block(src)
         mine = self._holds_block(src)
         lstart = list(bstart)
@@ -207,20 +190,20 @@ class RambaGroupby:
         local = torch.empty(max(n_loc, 1), dtype=tdt, device=RT.device)
         scratch = None
         if mine and bsize[ax] == 0:  # an empty grouped axis: every group is empty
-            local.fill_(_identity(op, is_f))
+            local.fill_(ident)
         elif mine:
-            view = advindex._local_view(src)
+            view = blocks.index_view(src)
             table = self._table(bstart[ax], bsize[ax])
             scratch = RT.group_reduce(view, rb_dtype(src.dtype), ax, table, op, center, local.data_ptr())
         if not cut:
-            return _Acc(local, lstart, _c_strides(lshape), code, (scratch,))
+            return _Acc(local, lstart, _contig_strides(lshape)[0], code, (scratch,))
         rshape = self._rshape(src.shape)
-        glob = torch.full((max(int(np.prod(rshape)), 1),), _identity(op, is_f), dtype=tdt, device=RT.device)
-        gst = _c_strides(rshape)
+        glob = torch.full((max(int(np.prod(rshape)), 1),), ident, dtype=tdt, device=RT.device)
+        gst = _contig_strides(rshape)[0]
         if n_loc:
             off = builtins.sum(s * st for s, st in zip(lstart, gst))
             RT.launch(_pack_program(code, code), lshape, [0] * len(lshape),
-                      [(local.data_ptr(), _c_strides(lshape), code), (glob.data_ptr() + off * 8, gst, code)])
+                      [(local.data_ptr(), _contig_strides(lshape)[0], code), (glob.data_ptr() + off * 8, gst, code)])
         RT.all_reduce(glob, _ALLREDUCE[op])
         return _Acc(glob, [0] * len(rshape), gst, code, (local, scratch))
 
@@ -261,7 +244,7 @@ class RambaGroupby:
         prog = _finish_program(kind, out_code, acc.code if acc is not None else cabi.F64)
         acc_ptr, acc_st = (acc.at(start), acc.strides) if acc is not None else (div[0], div[1])
         RT.launch(prog, list(shape), [0] * len(shape),
-                  [(out_ptr, _c_strides(shape), out_code, out_bounds), (acc_ptr, acc_st, acc.code if acc is not None else cabi.F64),
+                  [(out_ptr, _contig_strides(shape)[0], out_code, out_bounds), (acc_ptr, acc_st, acc.code if acc is not None else cabi.F64),
                    (div[0], div[1], cabi.F64)])
 
     def _result(self, src, cut, dtype):
@@ -281,7 +264,7 @@ class RambaGroupby:
                     size[ax], start[ax] = self.num_groups, 0
                 dist.append(shardview.shardview(np.array(size, dtype=np.int64), np.array(start, dtype=np.int64)))
             res = R.create_array_with_divisions(rshape, dist, dtype=dtype)
-        sh = advindex._shard(res)
+        sh = blocks.block(res)
         sv = res.distribution[common.worker_num]
         start = [int(x) for x in sv.start]
         shape = [int(x) for x in sv.size] if not shardview.is_empty(sv) else [0] * len(rshape)

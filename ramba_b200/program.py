@@ -49,6 +49,27 @@ def np_dtype(code):
     return _RB2NP[code]
 
 
+def getminmax(dtype):
+    dtype = np.dtype(dtype)
+    if dtype.kind == "f":
+        return (-np.inf, np.inf)
+    if dtype.kind == "b":
+        return (False, True)
+    i = np.iinfo(dtype)
+    return (i.min, i.max)
+
+
+def red_identity(op, dtype):
+    """The identity of reduction `op` (sum prod min max all any) over values of `dtype`: what an empty reduction starts
+    from and what a masked-out element contributes."""
+    if op in ("sum", "any"):
+        return 0
+    if op in ("prod", "all"):
+        return 1
+    lo, hi = getminmax(dtype)
+    return hi if op == "min" else lo
+
+
 def dtype_class(code):
     """Compute class an element of storage dtype `code` has inside the loop body."""
     if code == cabi.F64:

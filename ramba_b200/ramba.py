@@ -25,11 +25,12 @@ import torch
 
 from . import _cabi as cabi
 from . import advindex
+from . import blocks
 from . import common
 from . import shardview
 from .common import dprint, timer, add_time
-from .flush import _combine_program, _contig_strides, _local_shape, _pack_program, _plan_cache, run_deferred_ops
-from .program import E, Iota, Lowering, ProgramError, ProgramLimit, TempVar, dtype_class, rb_dtype
+from .flush import _combine_program, _contig_strides, _pack_program, _plan_cache, run_deferred_ops
+from .program import E, Iota, Lowering, ProgramError, ProgramLimit, TempVar, dtype_class, getminmax, rb_dtype, red_identity
 from .runtime import ALLREDUCE_OP, RT, torch_dtype
 
 int64 = np.int64
@@ -845,6 +846,18 @@ class DAG:
         deferred_op.do_ops()
 
     @classmethod
+    def before_write(cls, arr):
+        """Make arr's storage safe to overwrite outside a fused op: run every pending statement that reads it (WAR) and
+        the last one that writes it (WAW), then flush."""
+        g = arr.gid
+        nodes = list(cls.readers.get(g, ()))
+        if g in cls.last_writer:
+            nodes.append(cls.last_writer[g])
+        if nodes:
+            cls._run(nodes)
+        deferred_op.do_ops()
+
+    @classmethod
     def execute_all(cls, do_ops=False):
         """Run every pending node: start from the ones nothing depends on, oldest first, grouped by output shape
         (DAG.execute_all, ramba/ramba.py:5080-5105)."""
@@ -1232,7 +1245,7 @@ class ndarray:
             red_bcast = ndarray(self.shape, base=red_arr, distribution=bdist, local_border=0, readonly=False)
             tmp = deferred_op.get_temp_var()
             src = self
-            DAG.add([tmp, self if self.maskarray is None else E("where", self.maskarray, self, _identity_scalar(redop, dtype))],
+            DAG.add([tmp, self if self.maskarray is None else E("where", self.maskarray, self, red_identity(op, dtype))],
                                red_bcast, precode=[tmp, initval], postcode=[red_bcast, redop], elide=elide)
             return _reduction2b(red_arr, op, dtype, asarray)
         dsz, dist, bdist = shardview.reduce_axes(self.shape, self.distribution, axis)
@@ -1525,37 +1538,8 @@ def _raise_axis(a, nd):
     raise np.exceptions.AxisError(a, nd)
 
 
-def getminmax(dtype):
-    dtype = np.dtype(dtype)
-    if dtype.kind == "f":
-        return (-np.inf, np.inf)
-    if dtype.kind == "b":
-        return (False, True)
-    i = np.iinfo(dtype)
-    return (i.min, i.max)
-
-
-def _identity_scalar(redop, dtype):
-    if redop == cabi.RED_ADD:
-        return 0
-    if redop == cabi.RED_MUL:
-        return 1
-    mm = getminmax(dtype)
-    return mm[1] if redop == cabi.RED_MIN else mm[0]
-
-
 def _np_reduce(op):
     return {"sum": np.sum, "prod": np.prod, "min": np.min, "max": np.max, "all": np.all, "any": np.any}[op]
-
-
-def _host_identity(op, dtype):
-    dtype = np.dtype(dtype)
-    if op in ("sum", "any"):
-        return 0
-    if op in ("prod", "all"):
-        return 1
-    mm = getminmax(dtype)
-    return mm[1] if op == "min" else mm[0]
 
 
 def _local_partial_tensor(red_arr, n, op):
@@ -1564,9 +1548,10 @@ def _local_partial_tensor(red_arr, n, op):
     w = common.worker_num
     acc_dt = torch.float64 if red_arr.dtype.kind == "f" else torch.int64
     sv = red_arr.distribution[w]
-    if shardview.is_empty(sv) or red_arr.gid not in RT.shards:
-        return torch.full((n,), _host_identity(op, red_arr.dtype), dtype=acc_dt, device=RT.device)
-    return RT.shards[red_arr.gid].interior().reshape(-1)[:n].to(acc_dt)
+    sh = blocks.block(red_arr)
+    if shardview.is_empty(sv):
+        return torch.full((n,), red_identity(op, red_arr.dtype), dtype=acc_dt, device=RT.device)
+    return sh.interior().reshape(-1)[:n].to(acc_dt)
 
 
 def _reduction2b(red_arr, op, dtype, asarray):
@@ -1631,14 +1616,11 @@ def _reduction2(red_arr, op, redop, dtype, axis, keepdims):
         RT.all_reduce(t, op)
         out_shape = tuple(1 if d in axis else red_arr.shape[d] for d in range(nd))
         arr = ndarray(out_shape, dtype=red_arr.dtype, flex_dist=False)
-        sh = RT.create_array(arr.gid, _local_shape(arr.bdarray.distribution, w), arr.dtype, arr.bdarray.pad)
+        sh = blocks.block(arr)
         sv = arr.distribution[w]
         if not shardview.is_empty(sv):
             mine = t.view(out_shape)[shardview.to_slice(sv)]
-            n = int(np.prod([int(x) for x in sv.size]))
             sh.interior().copy_(mine)  # (converts the accumulator dtype back to the array's)
-        arr.bdarray.remote_constructed = True
-        arr.bdarray.flex_dist = False
         return arr if keepdims else arr[sl1]
     arr = empty_like(red_arr[sl2])
     name = {cabi.RED_ADD: "add", cabi.RED_MUL: "mul", cabi.RED_MIN: "min", cabi.RED_MAX: "max"}[redop]
@@ -1785,15 +1767,6 @@ for _n, (_r, _i, _d) in array_simple_reductions.items():
 # =============================================================================================
 # host <-> device edges
 # =============================================================================================
-def _shard_view_tensor(nd, w):
-    """torch view (this worker's part of `nd`, in view coordinates) of its shard."""
-    sv = nd.distribution[w]
-    sh = RT.shards[nd.gid]
-    box = shardview.clean_range(sv)
-    off, st = RT.bind_view(sv, sh.strides, box)
-    return sh.buf.as_strided([int(x) for x in sv.size], st, off + sh.origin) if builtins.min(st + [0]) >= 0 else None, off, st
-
-
 def _is_whole_shard(sv, sh):
     k = len(sv.size)
     return (k == len(sh.shape) and builtins.all(int(sv.axis_map[d]) == d and int(sv.steps[d]) == 1 and int(sv.base_offset[d]) == 0
@@ -1805,12 +1778,9 @@ def _part_to_host(nd, w, out=None, non_blocking=False):
     if nd.bdarray.failed is not None:
         _raise_failed(nd.bdarray)
     sv = nd.distribution[w]
+    sh = blocks.block(nd)  # (on every rank, also where the part is empty: the partition is fixed everywhere or nowhere)
     if shardview.is_empty(sv):
         return np.zeros([0] * nd.ndim, dtype=nd.dtype)
-    if nd.gid not in RT.shards:
-        bd = nd.bdarray
-        RT.create_array(nd.gid, _local_shape(bd.distribution, w), bd.dtype, bd.pad)
-    sh = RT.shards[nd.gid]
     shape = [int(x) for x in sv.size]
     if _is_whole_shard(sv, sh) and sh.border == 0 and nd.dtype != np.bool_:
         n = int(np.prod(shape))
@@ -1823,13 +1793,12 @@ def _part_to_host(nd, w, out=None, non_blocking=False):
         if host.data_ptr() == t.data_ptr():
             host = host.clone()  # (a host-resident shard: the caller gets a copy, never an alias of the live block)
         return host.numpy().reshape(shape)
-    bc = [int(a) < 0 for a in sv.axis_map]
-    cst, n = _contig_strides(shape, [False] * len(shape))
+    cst, n = _contig_strides(shape)
     buf = torch.empty(max(n, 1), dtype=torch_dtype(nd.dtype), device=RT.device)
-    off, st = RT.bind_view(sv, sh.strides, shardview.clean_range(sv))
+    ptr, st, _, _ = blocks.part(nd)
     code = rb_dtype(nd.dtype)
     RT.launch(_pack_program(code, code), shape, [0] * len(shape),
-              [(sh.ptr(off), st, code), (buf.data_ptr(), cst, code)])
+              [(ptr, st, code), (buf.data_ptr(), cst, code)])
     RT.synchronize()
     host = buf[:n].cpu().numpy().reshape(shape)
     if nd.dtype == np.bool_:
@@ -1892,9 +1861,8 @@ def fromarray(x, local_border=0, dtype=None, **kwargs):
         return array(x.astype(dtype))
     new = ndarray(x.shape, dtype=dtype, flex_dist=False, local_border=local_border, **kwargs)
     deferred_op.do_ops()
-    w = common.worker_num
-    sv = new.distribution[w]
-    sh = RT.create_array(new.gid, _local_shape(new.bdarray.distribution, w), new.dtype, new.bdarray.pad)
+    sv = new.distribution[common.worker_num]
+    sh = blocks.block(new)
     if not shardview.is_empty(sv):
         blk = x[shardview.to_slice(sv)]
         if blk.dtype != new.dtype:
@@ -1908,8 +1876,6 @@ def fromarray(x, local_border=0, dtype=None, **kwargs):
             sh.interior().copy_(t.view(sh.shape), non_blocking=True)
         else:
             sh.buf[: t.numel()].copy_(t, non_blocking=True)
-    new.bdarray.remote_constructed = True
-    new.bdarray.flex_dist = False
     return new
 
 
@@ -1922,9 +1888,8 @@ def fromarray_local(block, shape, dtype=None, **kwargs):
         dtype = block.dtype
     new = ndarray(shapeToInt(shape), dtype=dtype, flex_dist=False, **kwargs)
     deferred_op.do_ops()
-    w = common.worker_num
-    sv = new.distribution[w]
-    sh = RT.create_array(new.gid, _local_shape(new.bdarray.distribution, w), new.dtype, new.bdarray.pad)
+    sv = new.distribution[common.worker_num]
+    sh = blocks.block(new)
     if not shardview.is_empty(sv):
         if tuple(block.shape) != tuple(int(x) for x in sv.size):
             raise ValueError("fromarray_local: block shape %s != this rank's division %s" % (block.shape, tuple(int(x) for x in sv.size)))
@@ -1938,8 +1903,6 @@ def fromarray_local(block, shape, dtype=None, **kwargs):
             sh.interior().copy_(t.view(sh.shape), non_blocking=True)
         else:
             sh.buf[: t.numel()].copy_(t, non_blocking=True)
-    new.bdarray.remote_constructed = True
-    new.bdarray.flex_dist = False
     return new
 
 
@@ -2028,12 +1991,8 @@ _fill_programs = {}
 
 def _fill_now(nd, value):
     """Fill this worker's block of a brand-new array with a scalar, immediately."""
-    w = common.worker_num
-    bd = nd.bdarray
-    sv = bd.distribution[w]
-    sh = RT.create_array(nd.gid, _local_shape(bd.distribution, w), bd.dtype, bd.pad)
-    bd.remote_constructed = True
-    bd.flex_dist = False
+    sv = nd.bdarray.distribution[common.worker_num]
+    sh = blocks.block(nd)
     if shardview.is_empty(sv):
         return
     code = rb_dtype(nd.dtype)
@@ -2346,14 +2305,11 @@ def reshape_copy(arr, newshape):
     DAG.instantiate(src)
     W, w = common.num_workers, common.worker_num
     sdist, ddist = src.bdarray.distribution, out.bdarray.distribution
-    sh_src = RT.shards.get(src.gid) or RT.create_array(src.gid, _local_shape(sdist, w), src.dtype, src.bdarray.pad)
-    sh_dst = RT.create_array(out.gid, _local_shape(ddist, w), out.dtype, out.bdarray.pad)
-    out.bdarray.remote_constructed = True
-    out.bdarray.flex_dist = False
+    sh_src, sh_dst = blocks.block(src), blocks.block(out)
     if arr.size == 0:
         return out
     code = rb_dtype(arr.dtype)
-    isz = np.dtype(np.uint8 if arr.dtype == np.bool_ else arr.dtype).itemsize
+    isz = blocks.itemsize(arr.dtype)
     prog = _pack_program(code, code)
 
     def runs(shape, dist, r, shard):
@@ -2406,7 +2362,7 @@ def reshape_copy(arr, newshape):
         wk.wait()  # (the launching stream waits; the host does not)
     for (pl, so, do, buf) in unpack:
         copy_groups(pl, so, do, buf.data_ptr(), sh_dst.ptr(0), None, sh_dst.bounds)
-    RT.keepalive = [b for (_, b, _) in ops]
+    RT.hold(*[b for (_, b, _) in ops])
     return out
 
 
@@ -2875,12 +2831,9 @@ def _scan_native(a, axis, op, dtype):
             if builtins.any(int(sv.start[d]) != 0 or int(sv.size[d]) != src.shape[d] for d in range(nd) if d != axis):
                 return None
     res = create_array_with_divisions(src.shape, dist, dtype=out_dtype)
-    sh_src = RT.shards.get(src.gid) or RT.create_array(src.gid, _local_shape(dist, w), src.dtype, src.bdarray.pad)
-    sh_res = RT.create_array(res.gid, _local_shape(res.bdarray.distribution, w), res.dtype)
+    sh_src, sh_res = blocks.block(src), blocks.block(res)
     if sh_src.border:
         return None
-    res.bdarray.remote_constructed = True
-    res.bdarray.flex_dist = False
     lshape = sh_src.shape
     mine_empty = shardview.is_empty(dist[w])
     n_outer = int(np.prod(lshape[:axis])) if not mine_empty else 0
@@ -2891,9 +2844,10 @@ def _scan_native(a, axis, op, dtype):
     ncols = int(np.prod([src.shape[d] for d in range(nd) if d != axis]))
     totals = torch.empty(max(1, ncols), dtype=acc_dt, device=RT.device) if split_axis else None
     if totals is not None:
-        totals.fill_(_host_identity({cabi.RED_ADD: "sum", cabi.RED_MUL: "prod", cabi.RED_MIN: "min", cabi.RED_MAX: "max"}[op], out_dtype))
+        totals.fill_(red_identity({cabi.RED_ADD: "sum", cabi.RED_MUL: "prod", cabi.RED_MIN: "min", cabi.RED_MAX: "max"}[op], out_dtype))
+    scratch = carry = None
     if not mine_empty:
-        RT.cumulative(sh_src.ptr(0), sh_res.ptr(0), code, n_outer, length, n_inner, op, None, totals.data_ptr() if totals is not None else None)
+        scratch = RT.cumulative(sh_src.ptr(0), sh_res.ptr(0), code, n_outer, length, n_inner, op, None, totals.data_ptr() if totals is not None else None)
     if split_axis and W > 1:
         allt = torch.empty(W * ncols, dtype=acc_dt, device=RT.device)
         RT.all_gather(allt, totals).wait()
@@ -2907,7 +2861,7 @@ def _scan_native(a, axis, op, dtype):
                 # res[o, l, i] = carry[o, i] (op) res[o, l, i] for every l: one fused op with the carry broadcast along the axis
                 RT.launch(_combine_program(code, acc_code, op), [n_outer, length, n_inner], [0, 0, 0],
                           [(sh_res.ptr(0), [length * n_inner, n_inner, 1], code, sh_res.bounds), (carry.data_ptr(), [n_inner, 0, 1], acc_code)])
-                RT.keepalive_carry = carry
+    RT.hold(scratch, carry)  # (read only by the launches above)
     return res
 
 

@@ -171,7 +171,7 @@ class Runtime:
         self.bytes_sent = 0
         self.collectives = 0  # all-gather / all-reduce / broadcast calls issued
         self.ring_receives = 0  # halo pieces received into the ring of a padded block (getborder)
-        self.keepalive = None  # staging buffers of the last flush
+        self.held = ()  # see hold()
         self.profile_events = None  # list -> (start, end, n_insns) CUDA events around every launch
         self.on_reset = []  # the engine registers what else must be forgotten with the shards (pending DAG nodes, fused op)
 
@@ -202,11 +202,12 @@ class Runtime:
     def executor(self):
         return self.be().run
 
-    def _reduce_partials(self, *args):
-        return self.be().reduce_partials(*args)
-
-    def stream_handle(self):
-        return self.be().stream_handle()
+    def hold(self, *objs):
+        """Keep objs alive until the next hold: buffers that launches or transfers already enqueued on the current stream
+        still use.  Holding them is enough because the caching allocator hands a freed buffer out again in stream order;
+        a buffer that something not yet enqueued will read needs another owner.  Each hold replaces the last one (sync()
+        leaves them alone), so what is held never grows."""
+        self.held = objs
 
     def ensure_process_group(self):
         if common.num_workers <= 1 or self._pg_ready:
@@ -447,16 +448,42 @@ class Runtime:
         self.launches += 1
         return fop
 
+    # ---- the other kernels of the library, on the current stream.  Counting rule: `launches` counts one per call of a
+    # library entry point - a bound op list, a scan, a grouped reduction, a gather, a scatter, a route - whatever number of
+    # kernels the call runs; the fold of axis partials (reduce_partials) is not counted.  The methods that return a scratch
+    # buffer leave it to the caller to hold (hold()) past the call.
+    def reduce_partials(self, out_ptr, in_ptr, n, k, stride_k, code, rop):
+        """Fold k partial slices of n elements (stride_k apart) into out (rb200_reduce_partials)."""
+        be = self.be()
+        be.reduce_partials(out_ptr, in_ptr, n, k, stride_k, code, rop, be.stream_handle())
+
     def cumulative(self, src_ptr, dst_ptr, code, n_outer, length, n_inner, redop, carry_in=None, totals_out=None):
-        """Inclusive scan of one local block through the C-ABI (rb200_cumulative)."""
-        self.keepalive_scan = self.be().cumulative(src_ptr, dst_ptr, code, n_outer, length, n_inner, redop, carry_in, totals_out)
+        """Inclusive scan of one local block through the C-ABI (rb200_cumulative); returns the scratch buffer (or None)."""
+        scratch = self.be().cumulative(src_ptr, dst_ptr, code, n_outer, length, n_inner, redop, carry_in, totals_out)
         self.launches += 1
+        return scratch
 
     def group_reduce(self, view, src_code, axis, table, op, center, out):
         """Grouped reduction of one local view along `axis` through the C-ABI (rb200_group_reduce): out (device address,
         accumulator class) receives op over the members of every group (table: a cabi.GroupTable).  Returns the scratch
-        buffer (or None); the caller holds it until the launches that follow on this stream have been enqueued."""
+        buffer (or None)."""
         scratch = self.be().group_reduce(view, src_code, axis, table, op, center, out)
+        self.launches += 1
+        return scratch
+
+    def gather(self, view, lin, n, out, bad):
+        """out[i] = view[lin[i]] for n entries (rb200_gather; view: a cabi.IndexView); bad counts the out-of-range ones."""
+        self.be().gather(view, lin, n, out, bad)
+        self.launches += 1
+
+    def scatter(self, view, lin, n, values, bad):
+        """view[lin[i]] = values[i] for n entries (rb200_scatter); bad counts the out-of-range ones."""
+        self.be().scatter(view, lin, n, values, bad)
+        self.launches += 1
+
+    def route(self, table, lin, n, offsets, slots, counts, bad):
+        """Group n requests by owning rank (rb200_route; table: a cabi.RouteTable); returns the scratch buffer (or None)."""
+        scratch = self.be().route(table, lin, n, offsets, slots, counts, bad)
         self.launches += 1
         return scratch
 

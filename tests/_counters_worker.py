@@ -18,9 +18,9 @@ sys.path.insert(0, HERE)
 
 import numpy as onp  # noqa: E402
 
-import _index_vm  # noqa: E402
+import _oracle_backend  # noqa: E402
 
-_index_vm.install()  # the oracle backend, extended by the index kernels and the PHILOX draws
+_oracle_backend.install()
 
 import ramba_b200 as rb  # noqa: E402
 from ramba_b200 import common, flush  # noqa: E402

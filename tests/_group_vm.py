@@ -1,6 +1,6 @@
 """NumPy restatement of rb200_group_reduce and rb200_describe_group_plan (include/ramba_b200.h) on host pointers.  The GPU
 tests compare the CUDA library against it bit for bit, and the CPU tests run the engine's groupby through it
-(install(): the index oracle backend of _index_vm, which the binops' gather needs, plus group_reduce)."""
+(_oracle_backend.OracleBackend)."""
 import ctypes as C
 
 import numpy as np
@@ -172,20 +172,3 @@ def _library_accepts(view, src_code, axis, table, op, center, out):
     msg = lib.rb200_last_error().decode() if rc else ""
     assert rc == 0 or "no usable CUDA device" in msg, "libramba_b200 would reject this grouped reduction: " + msg
 
-
-def install():
-    """The index oracle backend (_index_vm.install) extended by group_reduce on host buffers."""
-    from ramba_b200.runtime import RT
-
-    _index_vm.install()
-    base = type(RT.backend)
-
-    class GroupOracleBackend(base):
-        def group_reduce(self, view, src_code, axis, table, op, center, out):
-            _library_accepts(view, src_code, axis, table, op, center, out)
-            group_reduce(view, src_code, axis, table, op, center, out)
-            return None
-
-    vm = RT.backend._vm
-    RT.backend = GroupOracleBackend()
-    RT.backend._vm = vm

@@ -30,11 +30,11 @@ def programs():
 def main():
     import faulthandler
 
-    import _group_vm
+    import _oracle_backend
 
     faulthandler.dump_traceback_later(int(os.environ.get("RB200_MR_WATCHDOG", "240")), exit=True)
     if (sys.argv[2] if len(sys.argv) > 2 else "oracle") == "oracle":
-        _group_vm.install()
+        _oracle_backend.install()
     import ramba_b200 as rb
     from ramba_b200 import common
     from ramba_b200.runtime import RT

@@ -1,6 +1,6 @@
 """NumPy restatement of rb200_gather, rb200_scatter and rb200_route (include/ramba_b200.h) on host pointers.  The GPU
 tests compare the CUDA library against it bit for bit, and the CPU tests run the engine's integer-array indexing through
-it (IndexOracleBackend)."""
+it (_oracle_backend.OracleBackend)."""
 import ctypes as C
 
 import numpy as np
@@ -118,23 +118,3 @@ def route(table, lin_ptr, n, offsets_ptr, slots_ptr, counts_ptr, bad_ptr):
         _host(offsets_ptr, nv, np.int64)[:] = off[order[:nv]]
     _host(bad_ptr, 1, np.uint64)[0] += np.uint64(n - nv)
 
-
-def install():
-    """Put the oracle backend, extended by gather / scatter / route on host buffers, under the engine."""
-    import _oracle_backend
-    from ramba_b200.runtime import RT
-
-    class IndexOracleBackend(_oracle_backend.OracleBackend):
-        def gather(self, view, lin, n, out, bad):
-            gather(view, lin, n, out, bad)
-
-        def scatter(self, view, lin, n, values, bad):
-            scatter(view, lin, n, values, bad)
-
-        def route(self, table, lin, n, offsets, slots, counts, bad):
-            route(table, lin, n, offsets, slots, counts, bad)
-
-    RT.backend = IndexOracleBackend()
-    import _philox_vm
-
-    RT.backend._vm = _philox_vm  # (the oracle extended by the PHILOX draws of random.choice)

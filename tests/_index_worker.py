@@ -73,11 +73,11 @@ def run_case(rb, name, shape, view, index, dtype, form, local_border=0):
 def main():
     import faulthandler
 
-    import _index_vm
+    import _oracle_backend
 
     faulthandler.dump_traceback_later(int(os.environ.get("RB200_MR_WATCHDOG", "240")), exit=True)
     if (sys.argv[2] if len(sys.argv) > 2 else "oracle") == "oracle":
-        _index_vm.install()
+        _oracle_backend.install()
     import ramba_b200 as rb
     from ramba_b200 import common
     from ramba_b200.runtime import RT

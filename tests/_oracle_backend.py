@@ -1,6 +1,8 @@
 """TEST-ONLY: run the engine's op lists through the NumPy oracle on host buffers, so that the
 fuser / partitioner / exchange logic can be exercised without a GPU.  The product never does
-this (ramba_b200.runtime raises without CUDA)."""
+this (ramba_b200.runtime raises without CUDA).  Op lists go through the oracle extended by the
+PHILOX draws (_philox_vm); gather, scatter, route and the grouped reduction through the NumPy
+restatements of those kernels (_index_vm, _group_vm)."""
 import os
 import sys
 
@@ -44,11 +46,12 @@ class OracleBackend:
 
     def __init__(self):
         import torch
-        from oracle import vm
+
+        import _philox_vm
 
         self.device = torch.device("cpu")
-        self.reduce_partials = vm.reduce_partials
-        self._vm = vm
+        self.reduce_partials = _philox_vm.reduce_partials
+        self._vm = _philox_vm
 
     def run(self, fop, stream=None):
         _library_accepts(fop)
@@ -70,6 +73,29 @@ class OracleBackend:
 
     def cumulative(self, src_ptr, dst_ptr, code, n_outer, length, n_inner, redop, carry_in, totals_out):
         self._vm.cumulative(src_ptr, dst_ptr, code, n_outer, length, n_inner, redop, carry_in, totals_out, None, None)
+        return None
+
+    def gather(self, view, lin, n, out, bad):
+        import _index_vm
+
+        _index_vm.gather(view, lin, n, out, bad)
+
+    def scatter(self, view, lin, n, values, bad):
+        import _index_vm
+
+        _index_vm.scatter(view, lin, n, values, bad)
+
+    def route(self, table, lin, n, offsets, slots, counts, bad):
+        import _index_vm
+
+        _index_vm.route(table, lin, n, offsets, slots, counts, bad)
+        return None
+
+    def group_reduce(self, view, src_code, axis, table, op, center, out):
+        import _group_vm
+
+        _group_vm._library_accepts(view, src_code, axis, table, op, center, out)
+        _group_vm.group_reduce(view, src_code, axis, table, op, center, out)
         return None
 
     def init_process_group(self):

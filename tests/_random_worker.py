@@ -11,8 +11,6 @@ sys.path.insert(0, HERE)
 
 import numpy as onp  # noqa: E402
 
-import _philox_vm  # noqa: E402
-
 MODE = sys.argv[2] if len(sys.argv) > 2 else "oracle"
 if MODE == "oracle":
     import _oracle_backend  # noqa: E402
@@ -22,9 +20,6 @@ if MODE == "oracle":
 import ramba_b200 as rb  # noqa: E402
 from ramba_b200 import common  # noqa: E402
 from ramba_b200.runtime import RT  # noqa: E402
-
-if MODE == "oracle":
-    RT.backend._vm = _philox_vm
 
 # GPU mode: every form over ragged 1-D, 2-D and 3-D shapes (the fill kernel, or the interpreter with RB200_NO_RNG=1)
 GPU_SHAPES = [(1000003,), (517, 301), (7, 33, 65)]

@@ -21,12 +21,13 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 
 @pytest.fixture
 def index_engine():
+    import _oracle_backend
     from ramba_b200 import ramba
     from ramba_b200.runtime import RT
 
     ramba.deferred_op.ramba_deferred_ops = None
     RT.reset()
-    V.install()
+    _oracle_backend.install()
     yield
     ramba.deferred_op.ramba_deferred_ops = None
     RT.reset()
@@ -131,8 +132,8 @@ def test_ordering_with_pending_statements(mode, tmp_path):
 import sys
 sys.path.insert(0, %r); sys.path.insert(0, %r)
 import numpy as onp
-import _index_vm
-_index_vm.install()
+import _oracle_backend
+_oracle_backend.install()
 import ramba_b200 as rb
 for rep in range(2):
     a = rb.fromarray(onp.arange(10.0))

@@ -22,12 +22,13 @@ AGGS = GW.AGGS
 
 @pytest.fixture
 def group_engine():
+    import _oracle_backend
     from ramba_b200 import ramba
     from ramba_b200.runtime import RT
 
     ramba.deferred_op.ramba_deferred_ops = None
     RT.reset()
-    GV.install()
+    _oracle_backend.install()
     yield
     ramba.deferred_op.ramba_deferred_ops = None
     RT.reset()

@@ -82,9 +82,7 @@ def test_key_derivation_is_pinned():
 @pytest.fixture
 def engine(oracle_engine):
     import _oracle_backend
-    from ramba_b200.runtime import RT
 
-    RT.backend._vm = P
     del _oracle_backend.PLANS[:]
     return _oracle_backend.PLANS
 
@@ -340,10 +338,9 @@ def test_fused_draws_plan_on_the_interpreter(engine):
 
 def test_rng_kill_switch_falls_back_to_the_interpreter():
     code = ("import sys; sys.path[:0] = [%r, %r]\n"
-            "import _oracle_backend, _philox_vm\n"
-            "from ramba_b200.runtime import RT\n"
+            "import _oracle_backend\n"
             "import ramba_b200 as rb\n"
-            "_oracle_backend.install(); RT.backend._vm = _philox_vm\n"
+            "_oracle_backend.install()\n"
             "rb.random.seed(1); rb.random.random((30, 20)).asarray()\n"
             "print(_oracle_backend.PLANS[-1])\n") % (ROOT, HERE)
     env = dict(os.environ, RB200_NO_RNG="1")
