@@ -1,11 +1,12 @@
 """ramba_b200.flush — this rank's share of one flush (RemoteState.run_deferred_ops, ramba/ramba.py:3493-3819).
 
-run_deferred_ops allocates the shards a fused op touches on first use, classifies every operand view as local / partly
-remote (is_compat / get_overlaps / intersect, ramba/ramba.py:3558-3644), brings the remote pieces through the runtime's
-transfers (halo pieces by one grouped send / receive, operands every rank needs whole by one all-gather), cuts the
-iteration box into ranges in which every operand has exactly one source (get_range_splits_list,
-ramba/ramba.py:3698-3706) and launches the op list once per range.  The first flush with a given key is recorded as a
-script (_FlushTape) that later flushes with the same key replay (_replay_tape).
+run_deferred_ops allocates the shards a fused op touches on first use and runs the flush's script.  The first flush with
+a given key plans that script (_plan, recorded on a _FlushTape) without launching or transferring anything: it
+classifies every operand view as local / partly remote (is_compat / get_overlaps / intersect,
+ramba/ramba.py:3558-3644), brings the remote pieces through the runtime's transfers (halo pieces by one grouped send /
+receive, operands every rank needs whole by one all-gather), cuts the iteration box into ranges in which every operand
+has exactly one source (get_range_splits_list, ramba/ramba.py:3698-3706) and launches the op list once per range.  One
+runner (_replay_tape) executes every flush, the first with its key as well as the later ones.
 
 The helpers the array code shares with it (_local_shape, _pack_program, _combine_program, _contig_strides) live here
 too.  Everything a flush needs is handed to it (the view table holds each operand's bdarray), so this module depends on
@@ -148,24 +149,22 @@ def _ring_receivable(bd_dist, vd, exec_dist, w, W, shard):
     return True
 
 
-_plan_cache = {}  # flush key -> script (_FlushTape)
+_plan_cache = {}  # flush key -> script (_FlushTape.finish)
 
 
 class _FlushTape:
-    """Everything a flush does to the GPU and to the other ranks, as it is done AND as a script: buffer allocations,
-    launches (the bound rb200_fused_op with its pointers replaced by (resource, byte offset) pairs: a resource is the
-    shard of one of the flush's views or one of the buffers the flush allocated), the all-gather, the grouped sends /
-    receives, the points where the launching stream waits for them, the fold of axis partials.  A later flush with the
-    same key (op list, partitions of the op and of every operand, shard layouts) replays the script instead of planning
-    again: pack -> P2P -> interior ranges -> wait -> boundary ranges becomes a loop over prepared structs
-    (`_replay_tape`); the plain flush (one range, all local) is a script of one launch.  RB200_VERIFY_PLAN_CACHE=1:
-    every hit plans again and the new script must be identical to the memoised one."""
+    """The script of one flush, recorded by _plan without launching or transferring anything: buffer allocations, launches
+    (the bound rb200_fused_op with its pointers replaced by (resource, byte offset) pairs: a resource is the shard of one
+    of the flush's views or one of the buffers the script allocates), the all-gather, the grouped sends / receives, the
+    points where the launching stream waits for them, the fold of axis partials.  The buffers are real only so that
+    _resolve can name the addresses bound into a launch; nothing is enqueued on them, and they die with the planner."""
 
     def __init__(self, shards):
         self.shards = shards
         self.actions = []
         self.buffers = []
         self.ring_receives = 0  # halo pieces received into the ring of a padded block (a placement, not a transfer)
+        self.in_flight = False  # transfers recorded and not yet waited for
 
     # ---- resources
     def _resolve(self, p):
@@ -191,7 +190,7 @@ class _FlushTape:
         return t
 
     def launch(self, *args, **kw):
-        fop = RT.launch(*args, submit=False, **kw)
+        fop = RT.bind(*args, **kw)
         patches = []
         for v in range(fop.n_views):
             one = fop.views[v]
@@ -206,11 +205,10 @@ class _FlushTape:
         scratch = self._resolve(fop.red_scratch)
         fop.red_scratch = 0
         self.actions.append(("launch", ctypes.string_at(ctypes.addressof(fop), ctypes.sizeof(fop)), tuple(patches), tuple(rp), scratch))
-        _submit_patched(self.actions[-1], self.shards, self.buffers)
 
     def all_gather(self, full, mine):
         self.actions.append(("allgather", self._slot(full), self._slot(mine)))
-        return RT.all_gather(full, mine)
+        self.in_flight = True
 
     def _slot(self, t):
         for k, b in enumerate(self.buffers):
@@ -219,23 +217,20 @@ class _FlushTape:
         raise ProgramError("internal: a transfer buffer the flush did not allocate")
 
     def p2p(self, ops):
-        """ops: [(is_send, buffer, peer)] -> the works of ONE grouped launch."""
+        """ops: [(is_send, buffer, peer)], sent / received by ONE grouped launch."""
         self.actions.append(("p2p", tuple([(bool(s), self._slot(b), int(peer)) for (s, b, peer) in ops])))
-        return RT.p2p(ops)
+        self.in_flight = True
 
-    def wait(self, works):
-        if works:
+    def wait(self):
+        """The launching stream waits for the transfers in flight; the host does not."""
+        if self.in_flight:
             self.actions.append(("wait",))
-            for wk in works:
-                wk.wait()  # the launching stream waits for the transfers; the host does not
+            self.in_flight = False
 
     def reduce_partials(self, out_ptr, in_ptr, n, k, stride_k, code, rop):
         self.actions.append(("fold", self._resolve(out_ptr), self._resolve(in_ptr), int(n), int(k), int(stride_k), int(code), int(rop)))
-        RT.reduce_partials(out_ptr, in_ptr, n, k, stride_k, code, rop)
 
     def finish(self):
-        RT.ring_receives += self.ring_receives
-        RT.hold(*self.buffers)  # consumed on the launching stream
         return (tuple(self.actions), self.ring_receives)
 
 
@@ -248,22 +243,18 @@ def _addr(res, shards, bufs):
     return RT.red_scratch().data_ptr()
 
 
-def _submit_patched(action, shards, bufs):
-    _, template, patches, rp, scratch = action
-    views = [(_addr(res, shards, bufs), shards[res[1]].bounds if bounded else None) for res, bounded in patches]
-    outs = [None if res is None else _addr(res, shards, bufs) for res in rp]
-    RT.submit(fill_template(template, views, outs, None if scratch is None else _addr(scratch, shards, bufs)))
-
-
 def _replay_tape(script, shards):
-    """Run a memoised flush script against this flush's shards (see _FlushTape)."""
+    """Execute a flush script (_FlushTape) against this flush's shards: the one code that runs a flush."""
     actions, ring_receives = script
     bufs = []
     works = []
     for a in actions:
         k = a[0]
         if k == "launch":
-            _submit_patched(a, shards, bufs)
+            _, template, patches, rp, scratch = a
+            views = [(_addr(res, shards, bufs), shards[res[1]].bounds if bounded else None) for res, bounded in patches]
+            outs = [None if res is None else _addr(res, shards, bufs) for res in rp]
+            RT.submit(fill_template(template, views, outs, None if scratch is None else _addr(scratch, shards, bufs)))
         elif k == "alloc":
             bufs.append(torch.empty(a[1], dtype=a[2], device=RT.device))
         elif k == "p2p":
@@ -279,6 +270,8 @@ def _replay_tape(script, shards):
     for wk in works:
         wk.wait()
     RT.ring_receives += ring_receives
+    # staging buffers are torch allocations consumed on the launching stream: the caching allocator reuses them in
+    # stream order, so no host synchronisation is needed here
     RT.hold(*bufs)
 
 
@@ -286,7 +279,6 @@ def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
     """This worker's share of one flush (RemoteState.run_deferred_ops, ramba/ramba.py:3493-3819).  views: the fuser's
     view table, (gid, operand) pairs; an operand has the view's shape, dtype and distribution and its bdarray as `bd`."""
     w, W = common.worker_num, common.num_workers
-    subspace = shardview.clean_range(exec_dist[w])
     # allocate shards on first touch
     shards = []
     for (gid, det) in views:
@@ -295,33 +287,65 @@ def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
         if sh is None:
             sh = RT.create_array(gid, _local_shape(bd.distribution, w), bd.dtype, bd.pad)
         shards.append(sh)
-    nviews = len(views)
-    vdist = [det.distribution for (_, det) in views]
     # ---- flush memo: apart from the buffer addresses, everything a flush does is a function of (op list, partitions of
-    # the op and of every operand, shard layouts).  The first execution is recorded as a script of allocations / launches
-    # / transfers / waits with symbolic addresses (_FlushTape); later executions replay it.
-    pkey = (prog, w, W, tuple([sv.key() for sv in exec_dist]), tuple([tuple([sv.key() for sv in vd]) for vd in vdist]),
+    # the op and of every operand, shard layouts).  A flush is planned into a script of allocations / launches /
+    # transfers / waits with symbolic addresses (_plan) once per key; every flush runs its key's script.
+    pkey = (prog, w, W, tuple([sv.key() for sv in exec_dist]), tuple([tuple([sv.key() for sv in det.distribution]) for (_, det) in views]),
             tuple([(sh.shape, sh.border) for sh in shards]), tuple(red_axes) if red_axes else (),
             # (what the ring of a padded block can receive depends on the partition of the whole array)
             tuple([tuple([sv.key() for sv in det.bd.distribution]) if sh.border else None
                    for (_, det), sh in zip(views, shards)]) if W > 1 else ())
-    memo = _plan_cache.get(pkey)
-    if memo is not None and not _VERIFY_PLAN_CACHE:
-        _replay_tape(memo, shards)
-        return
-    tape = _FlushTape(shards)
-
-    def _done():
-        script = tape.finish()
-        if memo is None:
+    script = _plan_cache.get(pkey)
+    if script is None or _VERIFY_PLAN_CACHE:
+        planned = _plan(views, shards, prog, exec_dist, gred, ared, red_axes)
+        if script is None:
             if len(_plan_cache) >= 1024:
                 _plan_cache.clear()
-            _plan_cache[pkey] = script
-        elif script != memo:
+            _plan_cache[pkey] = planned
+        elif planned != script:
             raise AssertionError("flush-script memo: planning the same flush again gives a different script")
+        script = planned
+    _replay_tape(script, shards)
+
+
+class _Source:
+    """An operand's source over iteration box `box`: this rank's block `shard` through shardview `sv`, or the staging
+    buffer `buf` holding the box with element strides `cst`.  `received`: a range that reads it waits for the transfers."""
+
+    def __init__(self, box, code, shard=None, sv=None, buf=None, cst=None, received=False):
+        self.box, self.code, self.shard, self.sv, self.buf, self.cst, self.received = box, code, shard, sv, buf, cst, received
+
+    def bind(self, r):
+        """This source over range r (inside its box), as a bound view of RT.bind."""
+        if self.sv is not None:
+            off, st = RT.bind_view(self.sv, self.shard.strides, r)
+            return (self.shard.ptr(off), st, self.code, self.shard.bounds)
+        off = 0
+        for d in range(len(self.cst)):
+            off += int(r.start[d] - self.box.start[d]) * self.cst[d]
+        return (self.buf.data_ptr() + off * self.buf.element_size(), list(self.cst), self.code)
+
+
+def _packed(part, bc):
+    """(shape, element strides, element count) of box `part` of a view packed in C order, broadcast dims collapsed."""
+    shp = [1 if bc[d] else int(part.size[d]) for d in range(len(bc))]
+    cst, n = _contig_strides(shp, bc)
+    return shp, cst, n
+
+
+def _view_index(views, red_view):
+    return [j for j, (g, det) in enumerate(views) if g == red_view.gid and shardview.dist_is_eq(det.distribution, red_view.distribution)][0]
+
+
+def _plan(views, shards, prog, exec_dist, gred, ared, red_axes):
+    """The script (_FlushTape) of this rank's share of one flush.  Launches and transfers nothing."""
+    w, W = common.worker_num, common.num_workers
+    subspace = shardview.clean_range(exec_dist[w])
+    nviews = len(views)
+    vdist = [det.distribution for (_, det) in views]
+    tape = _FlushTape(shards)
     vcode = [rb_dtype(det.dtype) for (_, det) in views]
     written = [bool(prog.view_written.get(i)) for i in range(nviews)]
-    ared_views = set()
     # which views are aligned with the iteration box on every worker?
     local_everywhere = []
     clean_exec = [shardview.clean_range(exec_dist[j]) for j in range(W)]
@@ -336,12 +360,20 @@ def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
                     ok = False
                     break
         local_everywhere.append(ok)
-    # parts[i] = list of (box, data_ptr, elem_strides or None(shard-addressed), sv)
-    parts = [[] for _ in range(nviews)]
+
+    def copy_part(i, part, bc, buf, unpack=False):
+        """Launch arguments of the copy between box `part` of this rank's block of view i and the contiguous buffer
+        `buf` (_packed): block -> buffer, or buffer -> block when unpack."""
+        shp, cst, _ = _packed(part, bc)
+        off, st = RT.bind_view(vdist[i][w], shards[i].strides, part)
+        block = (shards[i].ptr(off), [0 if bc[d] else st[d] for d in range(len(bc))], vcode[i])
+        flat = (buf.data_ptr(), cst, vcode[i])
+        return _pack_program(vcode[i], vcode[i]), shp, [0] * len(shp), [flat, block] if unpack else [block, flat]
+
+    parts = [[] for _ in range(nviews)]  # parts[i]: the _Sources of view i
     gathered = set()         # views served whole by an all-gathered buffer
     ring = [False] * nviews  # views whose remote pieces are received into the ring of this rank's padded block
-    post_wait = []           # unpack launches that need the received data: (program, shape, bound views)
-    pending = []  # collectives / transfers in flight: waited for only before the first range that reads what they bring
+    post_wait = []           # unpack launches that need the received data (copy_part's launch arguments)
     if W > 1 and not builtins.all(local_everywhere):
         ops = []
         for i in range(nviews):
@@ -352,29 +384,22 @@ def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
             bc = [int(a) < 0 for a in vdist[i][0].axis_map]
             ring[i] = shards[i].border > 0 and not shardview.is_empty(subspace) and _ring_receivable(
                 views[i][1].bd.distribution, vdist[i], exec_dist, w, W, shards[i])
+            tdt = torch_dtype(views[i][1].dtype)
             g = _gatherable(vdist[i], exec_dist, bc, views[i][1].shape, W)
             if g is not None:
                 # every rank needs every rank's part of this (small) operand and the parts are equal consecutive
                 # chunks: ONE all-gather into a buffer that then serves the whole iteration box as a single source
                 # (the reference ships W*(W-1) pickled pieces, ramba/ramba.py:3646-3693)
-                n = g
-                tdt = torch_dtype(views[i][1].dtype)
-                mine = tape.empty(n, tdt)
-                part = shardview.clean_range(vdist[i][w])
-                shp = [1 if bc[d] else int(part.size[d]) for d in range(len(bc))]
-                cst, _ = _contig_strides(shp, bc)
-                off, st = RT.bind_view(vdist[i][w], shards[i].strides, part)
-                tape.launch(_pack_program(vcode[i], vcode[i]), shp, [0] * len(shp),
-                            [(shards[i].ptr(off), [0 if bc[d] else st[d] for d in range(len(bc))], vcode[i]),
-                             (mine.data_ptr(), cst, vcode[i])])
-                full = tape.empty(W * n, tdt)
-                pending.append(tape.all_gather(full, mine))
+                mine = tape.empty(g, tdt)
+                tape.launch(*copy_part(i, shardview.clean_range(vdist[i][w]), bc, mine))
+                full = tape.empty(W * g, tdt)
+                tape.all_gather(full, mine)
                 vshape = views[i][1].shape
                 fshape = [1 if bc[d] else int(vshape[d]) for d in range(len(bc))]
                 fst, _ = _contig_strides(fshape, bc)
                 box = shardview.ShardView(np.array([int(subspace.size[d]) if bc[d] else int(vshape[d]) for d in range(len(bc))], dtype=np.int64),
                                           np.array([int(subspace.start[d]) if bc[d] else 0 for d in range(len(bc))], dtype=np.int64))
-                parts[i].append((box, full.data_ptr(), fst, None, True))
+                parts[i].append(_Source(box, vcode[i], buf=full, cst=fst, received=True))
                 gathered.add(i)
                 continue
             for peer in range(W):
@@ -385,61 +410,51 @@ def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
                 if not shardview.is_empty(pe) and not shardview.is_compat(pe, vdist[i][peer]):
                     part = shardview.intersect(vdist[i][w], exec_dist[peer])
                     if not shardview.is_empty(part):
-                        shp = [1 if bc[d] else int(part.size[d]) for d in range(len(bc))]
-                        cst, n = _contig_strides(shp, bc)
-                        buf = tape.empty(max(n, 1), torch_dtype(views[i][1].dtype))
-                        off, st = RT.bind_view(vdist[i][w], shards[i].strides, part)
-                        src_ptr = shards[i].ptr(off)
-                        tape.launch(_pack_program(vcode[i], vcode[i]), shp, [0] * len(shp),
-                                    [(src_ptr, [0 if bc[d] else st[d] for d in range(len(bc))], vcode[i]),
-                                     (buf.data_ptr(), cst, vcode[i])])
+                        buf = tape.empty(max(_packed(part, bc)[2], 1), tdt)
+                        tape.launch(*copy_part(i, part, bc, buf))
                         ops.append((True, buf, peer))
                 # what I need from `peer`
                 if not shardview.is_empty(subspace) and not shardview.is_compat(subspace, vdist[i][w]):
                     part = shardview.intersect(vdist[i][peer], exec_dist[w])
                     if not shardview.is_empty(part):
-                        shp = [1 if bc[d] else int(part.size[d]) for d in range(len(bc))]
-                        cst, n = _contig_strides(shp, bc)
-                        buf = tape.empty(max(n, 1), torch_dtype(views[i][1].dtype))
+                        _, cst, n = _packed(part, bc)
+                        buf = tape.empty(max(n, 1), tdt)
                         ops.append((False, buf, peer))
                         pb = shardview.clean_range(part)
                         if ring[i]:
                             # getborder (ramba/ramba.py:1260-1322): the neighbour's edge lands in the ring of MY padded
                             # block, where my own shardview of this view, extended past its box, addresses it
-                            off, st = RT.bind_view(vdist[i][w], shards[i].strides, pb)
-                            post_wait.append((_pack_program(vcode[i], vcode[i]), shp,
-                                              [(buf.data_ptr(), cst, vcode[i]), (shards[i].ptr(off), st, vcode[i])]))
-                            parts[i].append((pb, None, None, vdist[i][w], True))
+                            post_wait.append(copy_part(i, pb, bc, buf, unpack=True))
+                            parts[i].append(_Source(pb, vcode[i], shard=shards[i], sv=vdist[i][w], received=True))
                             tape.ring_receives += 1
                         else:
-                            parts[i].append((pb, buf.data_ptr(), cst, None, True))
+                            parts[i].append(_Source(pb, vcode[i], buf=buf, cst=cst, received=True))
         if ops:
             # the pack kernels run on the current stream; NCCL orders its transfers after them.  The transfers are NOT
             # waited for here: ranges whose operands are all local (the interior of a stencil) are launched first and
             # overlap with them (the reference sends, then blocks in the receive loop, ramba/ramba.py:3646-3693)
-            pending += tape.p2p(ops)
+            tape.p2p(ops)
     if shardview.is_empty(subspace):
-        tape.wait(pending)
-        _done()
-        return
+        tape.wait()
+        return tape.finish()
     # local parts
     for i in range(nviews):
         if i in gathered:
             continue
         sv = vdist[i][w]
         if local_everywhere[i] or shardview.is_compat(subspace, sv):
-            parts[i].append((subspace, None, None, sv, False))
+            parts[i].append(_Source(subspace, vcode[i], shard=shards[i], sv=sv))
         else:
             part = shardview.intersect(sv, exec_dist[w])
             if not shardview.is_empty(part):
-                parts[i].append((shardview.clean_range(part), None, None,
-                                 sv if ring[i] else shardview.mapslice_keep(sv, part.start, part.start + part.size), False))
+                parts[i].append(_Source(shardview.clean_range(part), vcode[i], shard=shards[i],
+                                        sv=sv if ring[i] else shardview.mapslice_keep(sv, part.start, part.start + part.size)))
     # ranges: every operand has one source inside a range
-    single = builtins.all(len(p) == 1 and not p[0][4] and (p[0][0] is subspace or shardview.is_compat(p[0][0], subspace)) for p in parts)
+    single = builtins.all(len(p) == 1 and not p[0].received and (p[0].box is subspace or shardview.is_compat(p[0].box, subspace)) for p in parts)
     if single:
         ranges = [subspace]
     else:
-        ranges = shardview.get_range_splits_list([shardview.clean_range(subspace)] + [p[0] for pl in parts for p in pl])
+        ranges = shardview.get_range_splits_list([shardview.clean_range(subspace)] + [s.box for p in parts for s in p])
         ranges = [r for r in ranges if not shardview.is_empty(r) and shardview.contains(subspace, r)]
     k = len(subspace.size)
     red_axes = list(red_axes) if red_axes else []
@@ -448,101 +463,80 @@ def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
     if gred:
         gred_out = [None] * len(prog.reds)
         for (slot, red_view) in gred:
-            i = [j for j, (g, det) in enumerate(views) if g == red_view.gid and shardview.dist_is_eq(det.distribution, red_view.distribution)][0]
+            i = _view_index(views, red_view)
             # this worker's element of the partial array: the first element of its (size-1) block
             off, _ = RT.bind_view(vdist[i][w], shards[i].strides, shardview.clean_range(vdist[i][w]))
             gred_out[slot] = (shards[i].ptr(off), vcode[i])
-    def _needs_transfer(r):
-        for i in range(nviews):
-            for (box, ptr, cst, sv, dep) in parts[i]:
-                if shardview.contains(box, r):
-                    if dep:
-                        return True
-                    break
-        return False
+    if ared:
+        ared = [(slot, _view_index(views, red_view)) for (slot, red_view, _) in ared]
 
-    if pending:
-        ranges = sorted(ranges, key=lambda r: 1 if _needs_transfer(r) else 0)  # (stable: local ranges first)
+    def source(i, r):
+        for s in parts[i]:
+            if shardview.contains(s.box, r):
+                return s
+        return None
+
+    def needs_transfer(r):
+        return builtins.any(s is not None and s.received for s in (source(i, r) for i in range(nviews)))
+
+    def wait_and_unpack():
+        tape.wait()
+        for args in post_wait:
+            tape.launch(*args)
+        post_wait.clear()
+
+    if tape.in_flight:
+        ranges = sorted(ranges, key=lambda r: 1 if needs_transfer(r) else 0)  # (stable: local ranges first)
     for r in ranges:
-        if pending and _needs_transfer(r):
-            tape.wait(pending)  # the launching stream waits for the transfers; the host does not
-            pending = []
-            for (pp, pshape, pbound) in post_wait:
-                tape.launch(pp, pshape, [0] * len(pshape), pbound)
-            post_wait = []
+        if tape.in_flight and needs_transfer(r):
+            wait_and_unpack()
         bound = []
-        ok = True
         for i in range(nviews):
-            src = None
-            if single:
-                src = parts[i][0]
-            else:
-                for (box, ptr, cst, sv, dep) in parts[i]:
-                    if shardview.contains(box, r):
-                        src = (box, ptr, cst, sv, dep)
-                        break
+            src = source(i, r)
             if src is None:
-                if ared and builtins.any(views[i][0] == rv.gid for (_, rv, _) in ared):
-                    src = None
-                ok = ok and (src is not None)
-                bound.append(None)
-                continue
-            box, ptr, cst, sv, dep = src
-            if sv is not None:
-                off, st = RT.bind_view(sv, shards[i].strides, r)
-                bound.append((shards[i].ptr(off), st, vcode[i], shards[i].bounds))
-            else:
-                off = 0
-                for d in range(k):
-                    off += int(r.start[d] - box.start[d]) * cst[d]
-                bound.append((ptr + off * np.dtype(views[i][1].dtype).itemsize, list(cst), vcode[i]))
-        if not ok:
-            raise ProgramError("internal: an operand has no source for range %r" % (r,))
+                raise ProgramError("internal: an operand has no source for range %r" % (r,))
+            bound.append(src.bind(r))
         shape_r = [int(x) for x in r.size]
         gs = [int(x) for x in r.start]
-        if not ared:
+        if ared:
+            _axis_reduction(tape, prog, ared, order, len(red_axes), shape_r, gs, bound, w, W)
+        else:
             tape.launch(prog, shape_r, gs, bound, reds=gred_out, worker_num=w, num_workers=W)
-            continue
-        # ---- axis reduction: stage 1 into per-split partials, then fold into the partial array
-        shape_p = [shape_r[d] for d in order]
-        gs_p = [gs[d] for d in order]
-        bound_p = [(b[0], [b[1][d] for d in order], b[2]) + tuple(b[3:]) for b in bound]
-        nred = len(red_axes)
-        kept_elems = 1
-        for d in range(nred, k):
-            kept_elems *= shape_p[d]
-        red_len = 1
-        for d in range(nred):
-            red_len *= shape_p[d]
-        kept_work = max(1, kept_elems // 4)
-        target = 132 * 2048  # H100 SXM: 132 SMs x 2048 resident threads
-        nsplit = 1 if kept_work >= target else builtins.min(builtins.max(1, red_len // 8), -(-target // kept_work))
-        nslots = len(prog.reds)
-        partials = tape.empty(nslots * nsplit * kept_elems + 1, torch.float64)
-        prog_p = _remap_iota(prog, order)
-        tape.launch(prog_p, shape_p, gs_p, bound_p, n_axis_red=nred, axis_nsplit=nsplit,
-                    axis_partials=partials.data_ptr(), worker_num=w, num_workers=W)
-        for (slot, red_view, redop) in ared:
-            rop, rct = prog.reds[slot]
-            acc_code = cabi.F64 if rct == cabi.T_F64 else cabi.I64
-            base = partials.data_ptr() + slot * nsplit * kept_elems * 8
-            tot_ptr = base
-            if nsplit > 1:
-                tot = tape.empty(kept_elems + 1, torch.float64)
-                tape.reduce_partials(tot.data_ptr(), base, kept_elems, nsplit, kept_elems, acc_code, rop)
-                tot_ptr = tot.data_ptr()
-            i = [j for j, (g, det) in enumerate(views) if g == red_view.gid and shardview.dist_is_eq(det.distribution, red_view.distribution)][0]
-            kept_shape = shape_p[nred:]
-            cst, _ = _contig_strides(kept_shape, [False] * len(kept_shape))
-            rb = bound_p[i]
-            tape.launch(_combine_program(vcode[i], acc_code, rop), kept_shape, gs_p[nred:],
-                        [(rb[0], rb[1][nred:], rb[2]), (tot_ptr, cst, acc_code)])
-    tape.wait(pending)  # (nothing needed them, e.g. an empty boundary)
-    for (pp, pshape, pbound) in post_wait:
-        tape.launch(pp, pshape, [0] * len(pshape), pbound)
-    # staging buffers are torch allocations consumed on the launching stream: the caching allocator reuses them in
-    # stream order, so no host synchronisation is needed here (the tape holds them until the next hold)
-    _done()
+    wait_and_unpack()  # (nothing needed them, e.g. an empty boundary)
+    return tape.finish()
+
+
+def _axis_reduction(tape, prog, ared, order, nred, shape_r, gs, bound, w, W):
+    """Axis reduction over one range: stage 1 (iteration dims permuted to `order`, the nred reduced dims first) into
+    per-split partials, then per (slot, view index of its partial array) in ared the fold of the splits and the combine."""
+    shape_p = [shape_r[d] for d in order]
+    gs_p = [gs[d] for d in order]
+    bound_p = [(b[0], [b[1][d] for d in order], b[2]) + tuple(b[3:]) for b in bound]
+    kept_elems = 1
+    for d in range(nred, len(order)):
+        kept_elems *= shape_p[d]
+    red_len = 1
+    for d in range(nred):
+        red_len *= shape_p[d]
+    kept_work = max(1, kept_elems // 4)
+    target = 132 * 2048  # H100 SXM: 132 SMs x 2048 resident threads
+    nsplit = 1 if kept_work >= target else builtins.min(builtins.max(1, red_len // 8), -(-target // kept_work))
+    partials = tape.empty(len(prog.reds) * nsplit * kept_elems + 1, torch.float64)
+    tape.launch(_remap_iota(prog, order), shape_p, gs_p, bound_p, n_axis_red=nred, axis_nsplit=nsplit,
+                axis_partials=partials.data_ptr(), worker_num=w, num_workers=W)
+    kept_shape = shape_p[nred:]
+    cst, _ = _contig_strides(kept_shape)
+    for (slot, i) in ared:
+        rop, rct = prog.reds[slot]
+        acc_code = cabi.F64 if rct == cabi.T_F64 else cabi.I64
+        tot_ptr = partials.data_ptr() + slot * nsplit * kept_elems * 8
+        if nsplit > 1:
+            tot = tape.empty(kept_elems + 1, torch.float64)
+            tape.reduce_partials(tot.data_ptr(), tot_ptr, kept_elems, nsplit, kept_elems, acc_code, rop)
+            tot_ptr = tot.data_ptr()
+        rb = bound_p[i]
+        tape.launch(_combine_program(rb[2], acc_code, rop), kept_shape, gs_p[nred:],
+                    [(rb[0], rb[1][nred:], rb[2]), (tot_ptr, cst, acc_code)])
 
 
 def _remap_iota(prog, order):

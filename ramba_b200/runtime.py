@@ -314,9 +314,13 @@ class Runtime:
         return off, strides
 
     # ---- launching ----------------------------------------------------------------------------
-    def launch(self, program, rng_shape, gstart, bound_views, reds=None, n_axis_red=0, axis_nsplit=1,
-               axis_partials=None, worker_num=0, num_workers=1, submit=True):
-        """Bind `program` to one range and call the C-ABI.
+    def launch(self, *args, **kw):
+        """submit(bind(...)): bind an op list to one range and hand it to the C-ABI."""
+        return self.submit(self.bind(*args, **kw))
+
+    def bind(self, program, rng_shape, gstart, bound_views, reds=None, n_axis_red=0, axis_nsplit=1,
+             axis_partials=None, worker_num=0, num_workers=1):
+        """Bind `program` to one range: the rb200_fused_op to submit.
         bound_views: list of (data_ptr, elem strides per iteration dim, rb dtype)."""
         # ---- launch memo: everything in the bound struct except the addresses is a function of (op list, range, strides)
         key = (program, tuple([int(s) for s in rng_shape]), tuple([int(g) for g in gstart]),
@@ -340,9 +344,7 @@ class Runtime:
             if len(_launch_cache) >= 4096:
                 _launch_cache.clear()
             _launch_cache[key] = ctypes.string_at(ctypes.addressof(fop), ctypes.sizeof(fop))
-        if not submit:
-            return fop
-        return self.submit(fop)
+        return fop
 
     def _build(self, program, rng_shape, gstart, bound_views, reds, n_axis_red, axis_nsplit, axis_partials, worker_num, num_workers):
         """Fill one rb200_fused_op from scratch (collapse / merge the iteration dims, copy the op list, bind the views)."""

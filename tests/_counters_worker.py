@@ -1,13 +1,14 @@
 """Worker process of tests/test_transfer_counters.py (RANK / WORLD_SIZE from the environment, gloo between the ranks, op
-lists through the oracle).  Runs every operation that talks to other ranks once, then again so that its flushes are
-replayed, and records how much RT.bytes_sent / RT.collectives grew each time next to what the counting rule of
-DESIGN.md §4 gives for the shapes and partitions involved:
+lists through the oracle).  Runs every operation that talks to other ranks once, then again so that its flushes run
+their memoised scripts, and records how much RT.bytes_sent / RT.collectives grew each time next to what the counting
+rule of DESIGN.md §4 gives for the shapes and partitions involved:
 
   grouped send / receive: the bytes of every send, no collective;  all-gather: 1 collective, bytes of this rank's part
   times W-1;  all-reduce: 1 collective, bytes of the tensor;  broadcast: 1 collective and, on the source rank only, bytes
   of the tensor times W-1.
 
-Prints one JSON line: {case: {"first": [bytes, collectives], "again": [...], "expected": [...], "replayed": n}}."""
+Prints one JSON line: {case: {"first": [bytes, collectives], "again": [...], "expected": [...], "planned": [flushes
+planned the first time, the second time]}}."""
 import json
 import os
 import sys
@@ -210,25 +211,27 @@ def main():
     # a rank that dies leaves the others waiting in a collective: dump the stack and exit instead of hanging
     faulthandler.dump_traceback_later(int(os.environ.get("RB200_MR_WATCHDOG", "240")), exit=True)
     RT.ensure_process_group()
-    flush._VERIFY_PLAN_CACHE = False  # the second runs must replay the scripts (verification mode plans them again)
-    replayed = [0]
-    replay = flush._replay_tape
+    flush._VERIFY_PLAN_CACHE = False  # the second runs must not plan the flushes again (verification mode does)
+    planned = [0]
+    plan = flush._plan
 
     def counted(*a, **k):
-        replayed[0] += 1
-        return replay(*a, **k)
+        planned[0] += 1
+        return plan(*a, **k)
 
-    flush._replay_tape = counted
+    flush._plan = counted
     out = {}
     for case in CASES:
         run = case()
         got = []
+        plans = []
         for _ in range(2):
-            replayed[0] = 0
+            planned[0] = 0
             b0, c0 = RT.bytes_sent, RT.collectives
             exp = run()
             got.append([RT.bytes_sent - b0, RT.collectives - c0])
-        out[case.__name__] = {"first": got[0], "again": got[1], "expected": list(exp), "replayed": replayed[0]}
+            plans.append(planned[0])
+        out[case.__name__] = {"first": got[0], "again": got[1], "expected": list(exp), "planned": plans}
     print(json.dumps(out))
     sys.stdout.flush()
     import torch.distributed as dist

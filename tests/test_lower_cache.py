@@ -129,8 +129,8 @@ def test_dtypes_are_part_of_the_key(verified_memo):
         assert got.dtype == exp.dtype and onp.array_equal(got, exp)
 
 
-# ---- the flush memo (flush.py::run_deferred_ops): every flush is recorded as a script, later flushes with the same key
-# replay it
+# ---- the flush memo (flush.py::run_deferred_ops): every flush is planned once per key into a script, and every flush
+# runs its key's script
 @pytest.fixture
 def verified_plans(oracle_engine, monkeypatch):
     from ramba_b200 import flush
@@ -140,17 +140,17 @@ def verified_plans(oracle_engine, monkeypatch):
     return flush
 
 
-def test_repeated_flush_is_replayed_from_its_script(verified_plans, monkeypatch):
+def test_repeated_flush_runs_its_script_without_planning_again(verified_plans, monkeypatch):
     import ramba_b200 as rb
 
     planned = []
-    orig = verified_plans._replay_tape
+    orig = verified_plans._plan
 
     def counted(*a, **k):
         planned.append(1)
         return orig(*a, **k)
 
-    monkeypatch.setattr(verified_plans, "_replay_tape", counted)
+    monkeypatch.setattr(verified_plans, "_plan", counted)
     x = onp.arange(5000, dtype=onp.float64) / 7.0
     A = rb.fromarray(x)
     U = rb.fromarray(onp.arange(20 * 30 * 40, dtype=onp.float32).reshape(20, 30, 40) % 17)
@@ -171,14 +171,14 @@ def test_repeated_flush_is_replayed_from_its_script(verified_plans, monkeypatch)
     for it in range(4):
         planned.clear()
         D, s = step()
-        assert len(planned) == (0 if it == 0 else 3), (it, len(planned))
+        assert len(planned) == (3 if it == 0 else 0), (it, len(planned))
         assert onp.allclose(D.asarray(), 1.0)
         assert s == float((x * 2.0 + 1.0).sum())
     # verified: planning each of the three flushes again must give its memoised script
     monkeypatch.setattr(verified_plans, "_VERIFY_PLAN_CACHE", True)
     planned.clear()
     D, s = step()
-    assert len(planned) == 0
+    assert len(planned) == 3
     assert onp.allclose(D.asarray(), 1.0)
     assert s == float((x * 2.0 + 1.0).sum())
     u = onp.asarray(U.asarray())
