@@ -177,7 +177,7 @@ def _lin(src_shape, terms, rshape, bpos, bshape):
         lin = R.create_array_with_divisions(rshape, part.distribution, dtype=np.int64)
     else:
         lin = R.empty(rshape, dtype=np.int64)
-    R.DAG.add([lin, expr], lin)
+    R.DAG.assign(lin, expr)
     return lin
 
 

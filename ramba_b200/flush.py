@@ -22,7 +22,7 @@ import torch
 from . import _cabi as cabi
 from . import common
 from . import shardview
-from .program import E, Lowering, ProgramError, rb_dtype
+from .program import E, REDUCTIONS, Lowering, ProgramError, rb_dtype
 from .runtime import RT, _VERIFY_PLAN_CACHE, fill_template, torch_dtype
 
 
@@ -41,13 +41,12 @@ def _pack_program(src_code, dst_code):
 _combine_programs = {}
 
 
-def _combine_program(red_code, acc_code, redop):
-    """red_view = red_view (op) partial  — applies stage-1 axis partials to the partial array."""
-    key = (red_code, acc_code, redop)
+def _combine_program(red_code, acc_code, combine):
+    """red_view = red_view (combine) partial  — applies stage-1 axis partials to the partial array."""
+    key = (red_code, acc_code, combine)
     if key not in _combine_programs:
         lw = Lowering([red_code, acc_code])
-        name = {cabi.RED_ADD: "add", cabi.RED_MUL: "mul", cabi.RED_MIN: "min", cabi.RED_MAX: "max"}[redop]
-        tv = lw.build(E(name, lw.read_view(0), lw.read_view(1)), None)
+        tv = lw.build(E(combine, lw.read_view(0), lw.read_view(1)), None)
         lw.store(0, tv)
         _combine_programs[key] = lw.finish()
     return _combine_programs[key]
@@ -275,7 +274,7 @@ def _replay_tape(script, shards):
     RT.hold(*bufs)
 
 
-def run_deferred_ops(uuid, views, prog, exec_dist, gred, ared, red_axes):
+def run_deferred_ops(views, prog, exec_dist, gred, ared, red_axes):
     """This worker's share of one flush (RemoteState.run_deferred_ops, ramba/ramba.py:3493-3819).  views: the fuser's
     view table, (gid, operand) pairs; an operand has the view's shape, dtype and distribution and its bdarray as `bd`."""
     w, W = common.worker_num, common.num_workers
@@ -468,7 +467,7 @@ def _plan(views, shards, prog, exec_dist, gred, ared, red_axes):
             off, _ = RT.bind_view(vdist[i][w], shards[i].strides, shardview.clean_range(vdist[i][w]))
             gred_out[slot] = (shards[i].ptr(off), vcode[i])
     if ared:
-        ared = [(slot, _view_index(views, red_view)) for (slot, red_view, _) in ared]
+        ared = [(slot, _view_index(views, red_view), REDUCTIONS[op].combine) for (slot, red_view, op) in ared]
 
     def source(i, r):
         for s in parts[i]:
@@ -508,7 +507,8 @@ def _plan(views, shards, prog, exec_dist, gred, ared, red_axes):
 
 def _axis_reduction(tape, prog, ared, order, nred, shape_r, gs, bound, w, W):
     """Axis reduction over one range: stage 1 (iteration dims permuted to `order`, the nred reduced dims first) into
-    per-split partials, then per (slot, view index of its partial array) in ared the fold of the splits and the combine."""
+    per-split partials, then per (slot, view index of its partial array, combine operator) in ared the fold of the splits
+    and the combine."""
     shape_p = [shape_r[d] for d in order]
     gs_p = [gs[d] for d in order]
     bound_p = [(b[0], [b[1][d] for d in order], b[2]) + tuple(b[3:]) for b in bound]
@@ -526,7 +526,7 @@ def _axis_reduction(tape, prog, ared, order, nred, shape_r, gs, bound, w, W):
                 axis_partials=partials.data_ptr(), worker_num=w, num_workers=W)
     kept_shape = shape_p[nred:]
     cst, _ = _contig_strides(kept_shape)
-    for (slot, i) in ared:
+    for (slot, i, combine) in ared:
         rop, rct = prog.reds[slot]
         acc_code = cabi.F64 if rct == cabi.T_F64 else cabi.I64
         tot_ptr = partials.data_ptr() + slot * nsplit * kept_elems * 8
@@ -535,7 +535,7 @@ def _axis_reduction(tape, prog, ared, order, nred, shape_r, gs, bound, w, W):
             tape.reduce_partials(tot.data_ptr(), tot_ptr, kept_elems, nsplit, kept_elems, acc_code, rop)
             tot_ptr = tot.data_ptr()
         rb = bound_p[i]
-        tape.launch(_combine_program(rb[2], acc_code, rop), kept_shape, gs_p[nred:],
+        tape.launch(_combine_program(rb[2], acc_code, combine), kept_shape, gs_p[nred:],
                     [(rb[0], rb[1][nred:], rb[2]), (tot_ptr, cst, acc_code)])
 
 

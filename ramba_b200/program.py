@@ -59,15 +59,32 @@ def getminmax(dtype):
     return (i.min, i.max)
 
 
+class Reduction:
+    """What one reduction means to each part of the engine.  code: the kernel's RED_* code (stage 1, partial folds,
+    the scan); combine: the E operator that folds two partials (stage 2, the scan's carry); allreduce: the
+    torch.distributed ReduceOp name; identity(dtype): what an empty reduction starts from and what a masked-out element
+    contributes; fold(stack): the torch fold of a stack of partials along dim 0 (the scan's carry); truth: the result
+    is a truth value (all / any reduce 0/1 values, so min / max all-reduce them)."""
+
+    __slots__ = ("code", "combine", "allreduce", "identity", "fold", "truth")
+
+    def __init__(self, code, combine, allreduce, identity, fold, truth=False):
+        self.code, self.combine, self.allreduce, self.identity, self.fold, self.truth = code, combine, allreduce, identity, fold, truth
+
+
+REDUCTIONS = {
+    "sum": Reduction(cabi.RED_ADD, "add", "SUM", lambda dt: 0, lambda s: s.sum(0)),
+    "prod": Reduction(cabi.RED_MUL, "mul", "PRODUCT", lambda dt: 1, lambda s: s.prod(0)),
+    "min": Reduction(cabi.RED_MIN, "min", "MIN", lambda dt: getminmax(dt)[1], lambda s: s.min(0).values),
+    "max": Reduction(cabi.RED_MAX, "max", "MAX", lambda dt: getminmax(dt)[0], lambda s: s.max(0).values),
+    "all": Reduction(cabi.RED_MUL, "mul", "MIN", lambda dt: 1, lambda s: s.min(0).values, truth=True),
+    "any": Reduction(cabi.RED_ADD, "add", "MAX", lambda dt: 0, lambda s: s.max(0).values, truth=True),
+}
+
+
 def red_identity(op, dtype):
-    """The identity of reduction `op` (sum prod min max all any) over values of `dtype`: what an empty reduction starts
-    from and what a masked-out element contributes."""
-    if op in ("sum", "any"):
-        return 0
-    if op in ("prod", "all"):
-        return 1
-    lo, hi = getminmax(dtype)
-    return hi if op == "min" else lo
+    """The identity of reduction `op` (sum prod min max all any) over values of `dtype`."""
+    return REDUCTIONS[op].identity(dtype)
 
 
 def dtype_class(code):
@@ -90,17 +107,6 @@ class Iota:
 
     def __init__(self, dim):
         self.dim = dim
-
-
-class TempVar:
-    """Scalar temporary of the loop body (deferred_op.temp_var, ramba/ramba.py:8090-8108)."""
-
-    __slots__ = ("name",)
-    _count = 0
-
-    def __init__(self):
-        TempVar._count += 1
-        self.name = "t%d" % TempVar._count
 
 
 class E:

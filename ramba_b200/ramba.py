@@ -5,11 +5,12 @@ shifted-slice path (SURVEY.md §8a):
 
   bdarray / ndarray        ramba/ramba.py:1049-1158, 5409-6901
   op tables + make_method  ramba/ramba.py:7842-7993
-  deferred_op              ramba/ramba.py:8039-8533  (add_op / do_ops / execute keep their call shape;
-                           the alternating "code string, operand" oplist becomes [dst, expression])
+  deferred_op              ramba/ramba.py:8039-8533  (do_ops / execute keep their call shape; add_op takes one
+                           Statement record instead of the alternating "code string, operand" oplist)
   creation / sync          ramba/ramba.py:8563-8991, 9843-9849
 
-API calls append statements to the current fused op; nothing runs until a flush (sync(),
+Each API call writes one Statement (`dst = expr`, or a reduction by op name over its axes) through DAG.assign /
+DAG.reduce; the DAG hands it to the current fused op; nothing runs until a flush (sync(),
 asarray(), a scalar read, or an incompatible op).  At flush, arrays whose Python handle is dead
 never touch HBM (they are register temporaries), live ones are read/written in place
 (ramba/ramba.py:8123-8127).  Execution is SPMD: every rank runs this driver code and executes its
@@ -30,8 +31,8 @@ from . import common
 from . import shardview
 from .common import dprint, timer, add_time
 from .flush import _combine_program, _contig_strides, _pack_program, _plan_cache, run_deferred_ops
-from .program import E, Iota, Lowering, ProgramError, ProgramLimit, TempVar, dtype_class, getminmax, rb_dtype, red_identity
-from .runtime import ALLREDUCE_OP, RT, torch_dtype
+from .program import E, REDUCTIONS, Iota, Lowering, ProgramError, ProgramLimit, dtype_class, getminmax, rb_dtype, red_identity
+from .runtime import RT, torch_dtype
 
 int64 = np.int64
 float64 = np.float64
@@ -128,7 +129,7 @@ class ArrRef:
     handle alive: whether a temporary is materialised depends on its handle being dead at flush
     time (ramba/ramba.py:8123-8127; the reference keeps only variable names + the bdarray)."""
 
-    __slots__ = ("gid", "distribution", "shape", "dtype", "local_border", "bd", "value")
+    __slots__ = ("gid", "distribution", "shape", "dtype", "local_border", "bd")
 
     def __init__(self, nd):
         self.gid = nd.gid
@@ -137,7 +138,6 @@ class ArrRef:
         self.dtype = nd.dtype
         self.local_border = nd.local_border
         self.bd = nd.bdarray
-        self.value = nd.distribution.item() if nd.shape == () else None
 
 
 def _raise_failed(bd):
@@ -145,44 +145,40 @@ def _raise_failed(bd):
 
 
 def _ref_of(nd):
-    """The ArrRef of a handle (one per handle: a handle's shape, partition and buffer never change; 0-d arrays hold a
-    mutable value and get a fresh one every time)."""
-    if nd.shape == ():
-        return ArrRef(nd)
+    """The ArrRef of a handle (one per handle: a handle's shape, partition and buffer never change)."""
     r = nd._ref
     if r is None:
         r = nd._ref = ArrRef(nd)
     return r
 
 
-def _detach(x):
+def _detach(x, reads, direct):
+    """The expression with every array leaf replaced by its ArrRef (the handle appended to `reads`, in order of appearance)
+    and every 0-d array leaf by the value it holds NOW (0-d arrays keep their value on the host and can be assigned to
+    before a deferred statement runs).  That value is a NumPy scalar in a statement the DAG defers and a Python scalar in
+    one that goes `direct`ly to the fuser: the lowering types a scalar by its type."""
     if isinstance(x, E):
-        return E(x.op, *[_detach(a) for a in x.args], imm=x.imm)
+        return E(x.op, *[_detach(a, reads, direct) for a in x.args], imm=x.imm)
     if isinstance(x, ndarray):
+        if x.shape == ():
+            return x.distribution.item() if direct else x.distribution[()]
+        reads.append(x)
         return _ref_of(x)
     return x
 
 
-def _array_operands(x, out):
-    """The non-0-d arrays an expression reads, in order of appearance."""
-    if isinstance(x, E):
-        for a in x.args:
-            _array_operands(a, out)
-    elif isinstance(x, ndarray):
-        if x.shape != ():
-            out.append(x)
-        else:
-            out.append(None)  # (marks a 0-d array leaf: DAG.add replaces those by their current values)
+class Statement:
+    """One deferred statement, as the API call wrote it.  An assignment (op None) is `dst = expr` at every index of dst,
+    where dst's mask (its maskarray) is true; a reduction is `dst = dst (op) expr` reduced over `axes` (None: every axis),
+    dst being the partial array's view broadcast to the source's shape.  expr is an E tree over ArrRefs, scalars and Iota;
+    `reads` holds the handles of its array operands, which keep them alive while the statement waits in the DAG.
+    deferred_op.add_op replaces dst and mask by their ArrRefs and drops `reads`: a pending fused op holds no handle."""
 
+    __slots__ = ("dst", "expr", "reads", "mask", "op", "axes", "elide")
 
-def _snapshot_0d(x):
-    """The expression with every 0-d array leaf replaced by the value it holds NOW (0-d arrays keep their value on the host
-    and can be assigned to before a deferred statement runs)."""
-    if isinstance(x, E):
-        return E(x.op, *[_snapshot_0d(a) for a in x.args], imm=x.imm)
-    if isinstance(x, ndarray) and x.shape == ():
-        return x.distribution[()]
-    return x
+    def __init__(self, dst, expr, reads, op=None, axes=None, elide=None):
+        self.dst, self.expr, self.reads, self.mask = dst, expr, reads, dst.maskarray
+        self.op, self.axes, self.elide = op, axes, elide
 
 
 def _walk_operands(x, out):
@@ -213,11 +209,7 @@ def _check_same_lowering(a, b):
 
 class deferred_op:
     ramba_deferred_ops = None
-    count = 0
     max_statements = 40
-
-    class temp_var(TempVar):
-        pass
 
     def __init__(self, shape, distribution, fdist):
         self.shape = shape
@@ -231,15 +223,9 @@ class deferred_op:
         self.use_gids = {}  # gid -> ([(view index within gid, details)], bd_shape, bd_distribution, pad, flex)
         self.preconstructed_gids = {}
         self.statements = []
-        self.axis_reductions = []
+        self.red_axes = None  # the axes every axis reduction of this op reduces over (ramba/ramba.py:8425-8432)
         self.keepalives = set()
         self.elide_gids = set()  # arrays proven unobservable after the flush (dying temporaries of a reduction)
-        self.uuid = "ramba_def_ops_%05d" % deferred_op.count
-        deferred_op.count += 1
-
-    @classmethod
-    def get_temp_var(cls):
-        return cls.temp_var()
 
     def add_gid(self, nd):
         gid = nd.bdarray.gid
@@ -258,33 +244,22 @@ class deferred_op:
 
     # ---- adding statements --------------------------------------------------------------
     @classmethod
-    def add_op(cls, oplist, write_array, imports=(), axis_reduce=None, precode=(), postcode=(), elide=None, _reads=None):
-        """oplist = [dst, expr]: `dst = expr` for every index of the iteration space.  dst is an
-        ndarray or a temp_var; expr is an E tree over ndarrays, scalars, temp_vars and Iota.
-        Global reductions pass precode=[tmp, init] and postcode=[red_array_view, redop-name]
-        (ramba/ramba.py:5798-5807); axis reductions pass axis_reduce=(axes, red_view)
-        (ramba/ramba.py:5809-5814).  `elide` names the gid of an operand that nobody can observe once the
-        calling API function returns (the temporary of `(X*2.0 + 1.0).sum()`): it is treated as dead in the flush
-        that holds this statement, provided the statement that writes it is part of the SAME fused op.
-        `_reads`: the non-0-d array operands of expr when the caller (the DAG node) has walked it already."""
+    def add_op(cls, stmt):
+        """Admit Statement `stmt` to the pending fused op, flushing that first if the two cannot fuse (the operator seam,
+        ramba/ramba.py:8383-8385).  A reduction's `elide` names the gid of an operand that nobody can observe once the
+        calling API function returns (the temporary of `(X*2.0 + 1.0).sum()`): it is treated as dead in the flush that
+        holds this statement, provided the statement that writes it is part of the SAME fused op."""
         t0 = timer()
-        dst, expr = oplist[0], oplist[1]
-        dst_nd = isinstance(dst, ndarray)
-        if _reads is None:
-            _reads = []
-            _array_operands(expr, _reads)
-            if None in _reads:
-                _reads = [o for o in _reads if o is not None]
-        operands = [dst] + _reads if dst_nd and dst.shape != () else _reads
-        arr = write_array
-        if arr is None:
-            arr = dst if dst_nd else next((o for o in _walk_operands(expr, []) if isinstance(o, ndarray)), None)
-        assert arr is not None, "Deferred op with no ndarray parameter"
-        shape, distribution = arr.shape, arr.distribution
-        abd = arr.bdarray
-        # the partition of `arr` can still follow the op's only if arr is a whole array that no flush has touched: a VIEW of
+        dst, reads = stmt.dst, stmt.reads
+        # (a global reduction only accumulates into its partial view, through a reduction slot: it neither reads nor
+        # stores that view element by element)
+        stores = stmt.op is None or stmt.axes is not None
+        operands = [dst] + reads if stores and dst.shape != () else reads
+        shape, distribution = dst.shape, dst.distribution
+        abd = dst.bdarray
+        # the partition of `dst` can still follow the op's only if dst is a whole array that no flush has touched: a VIEW of
         # a flexible array was cut from the partition the array had then and does not move when the array is pinned
-        fixed = abd.remote_constructed or not abd.flex_dist or arr.base is not None
+        fixed = abd.remote_constructed or not abd.flex_dist or dst.base is not None
         cur = cls.ramba_deferred_ops
         if cur is not None:
             if (cur.shape != shape
@@ -292,7 +267,7 @@ class deferred_op:
                     or len(cur.statements) >= cls.max_statements):
                 cls.do_ops()
                 cur = None
-            elif cur.axis_reductions and (axis_reduce is None or cur.axis_reductions[0][0] != list(axis_reduce[0])):
+            elif cur.red_axes is not None and stmt.axes != cur.red_axes:
                 # reductions on an axis must agree (ramba/ramba.py:8425-8432); a plain statement after an axis reduction
                 # would run once per reduced element
                 cls.do_ops()
@@ -314,8 +289,8 @@ class deferred_op:
                 cls.do_ops()
                 cur = None
         # alias check 2: writes an array that is also read through a different view
-        if write_array is not None and dst_nd:
-            wgid, wdist = write_array.bdarray.gid, write_array.distribution
+        if stores:
+            wgid, wdist = abd.gid, dst.distribution
             hit = False
             for o in operands:
                 if o is not dst and o.bdarray.gid == wgid and not shardview.dist_is_eq(o.distribution, wdist):
@@ -327,28 +302,27 @@ class deferred_op:
                         hit = True
                         break
             if hit:
-                tmp_array = empty_like(write_array)
-                cls.add_op([tmp_array, expr], tmp_array, imports)
+                tmp_array = empty_like(dst)
+                cls.add_op(Statement(tmp_array, stmt.expr, reads))
                 cls.do_ops()
-                cls.add_op([write_array, tmp_array], write_array)
+                cls.add_op(Statement(dst, _ref_of(tmp_array), [tmp_array]))
                 return
         if cur is None:
             cur = cls.ramba_deferred_ops = cls(shape, distribution, not fixed)
         if fixed and (cur.flex_dist or not abd.flex_dist):
             cur.distribution = distribution
             cur.flex_dist = False
+        elide = stmt.elide
         if elide is not None and elide in cur.write_gids and bdarray.valid_gid(elide) \
                 and not bdarray.get_by_gid(elide).remote_constructed:
             # (decided HERE, after admission: a flush forced by this very statement must still materialise the operand)
             cur.elide_gids.add(elide)
-        mask = None
-        if write_array is not None and dst_nd:
-            if write_array.maskarray is not None:
-                mask = write_array.maskarray
+        mask = stmt.mask
+        if stores:
+            if mask is not None:
                 operands = [mask] + operands
-            wbd = write_array.bdarray
-            cur.write_arrs.append((wbd.gid, None if wbd.flex_dist else write_array.distribution))
-            cur.write_gids.add(wbd.gid)
+            cur.write_arrs.append((abd.gid, None if abd.flex_dist else distribution))
+            cur.write_gids.add(abd.gid)
         read_arrs, read_gids = cur.read_arrs, cur.read_gids
         for x in operands:
             xbd = x.bdarray
@@ -357,18 +331,14 @@ class deferred_op:
             read_arrs.append((xbd.gid, None if xbd.flex_dist else x.distribution))
             read_gids.add(xbd.gid)
             cur.add_gid(x)
-        expr = _detach(expr)
-        if axis_reduce is not None:
-            axes, red_view = axis_reduce
-            cur.add_gid(red_view)
-            cur.axis_reductions.append((list(axes), ArrRef(red_view)))
-            cur.statements.append(("ared", postcode[1], expr, ArrRef(red_view)))
-        elif precode:
-            red_view = postcode[0]
-            cur.add_gid(red_view)
-            cur.statements.append(("gred", postcode[1], expr, ArrRef(red_view)))
-        else:
-            cur.statements.append(("assign", _detach(dst), expr, _detach(mask) if mask is not None else None))
+        if stmt.op is not None:
+            cur.add_gid(dst)
+            if stmt.axes is not None:
+                cur.red_axes = stmt.axes
+        stmt.dst = _ref_of(dst)
+        stmt.mask = _ref_of(mask) if mask is not None else None
+        stmt.reads = None
+        cur.statements.append(stmt)
         add_time("deferred_ops::add_op", timer() - t0)
 
     @classmethod
@@ -428,17 +398,12 @@ class deferred_op:
                 raise
             m = len(statements) // 2
             first, second = statements[:m], statements[m:]
-            written = set()
-            for st in first:
-                if st[0] == "assign" and isinstance(st[1], ArrRef):
-                    written.add(st[1].gid)
-                elif st[0] == "assign" and isinstance(st[1], TempVar):
-                    raise
+            written = {st.dst.gid for st in first if st.op is None}
             crossing = {}
             for st in second:
-                for x in (st[2], st[3] if st[0] == "assign" else None):
+                for x in (st.expr, st.mask):
                     for o in _walk_operands(x, []):
-                        if isinstance(o, ArrRef) and o.shape != () and o.gid in written and o.gid not in live_gids:
+                        if isinstance(o, ArrRef) and o.gid in written and o.gid not in live_gids:
                             crossing[o.gid] = self.use_gids[o.gid]
             self._pin(crossing)
             both = dict(live_gids)
@@ -456,8 +421,7 @@ class deferred_op:
         if common.debug_showcode and common.worker_num == 0:
             print(format_program(prog, views, self.shape))
         t1 = timer()
-        run_deferred_ops(self.uuid, views, prog, self.distribution, gred, ared,
-                         self.axis_reductions[0][0] if ared else None)
+        run_deferred_ops(views, prog, self.distribution, gred, ared, self.red_axes if ared else None)
         add_time("run_deferred_ops", timer() - t1)
 
     def _lower(self, statements, live_gids):
@@ -470,7 +434,6 @@ class deferred_op:
         vindex = {}
         reads = {}
         gid_ids = {}
-        tmp_ids = {}
         elide = self.elide_gids
 
         def view_of(nd):
@@ -488,15 +451,11 @@ class deferred_op:
             if isinstance(x, E):
                 return (x.op, x.imm) + tuple([key_of(a) for a in x.args])
             if isinstance(x, ArrRef):
-                if x.shape == ():
-                    return ("s", type(x.value), repr(x.value))
                 if x.gid in live_gids:
                     i = view_of(x)
                     reads[i] = reads.get(i, 0) + 1
                     return ("v", i)
                 return ("d", gid_ids.setdefault(x.gid, len(gid_ids)))
-            if isinstance(x, TempVar):
-                return ("t", tmp_ids.setdefault(x, len(tmp_ids)))
             if isinstance(x, Iota):
                 return ("i", x.dim)
             if isinstance(x, np.ndarray) and x.shape == ():
@@ -505,22 +464,19 @@ class deferred_op:
 
         skeys = []
         for st in statements:
-            if st[0] == "assign":
-                ek = key_of(st[2])
-                mk = key_of(st[3]) if st[3] is not None else None
-                dst = st[1]
-                if isinstance(dst, TempVar):
-                    dk = ("t", tmp_ids.setdefault(dst, len(tmp_ids)))
-                elif dst.gid in live_gids:
-                    dk = ("v", view_of(dst))
-                elif dst.gid in elide:
-                    dk = ("e", gid_ids.setdefault(dst.gid, len(gid_ids)), rb_dtype(dst.dtype))
-                else:
-                    dk = ("d", gid_ids.setdefault(dst.gid, len(gid_ids)))
-                skeys.append(("assign", dk, ek, mk))
+            ek = key_of(st.expr)
+            dst = st.dst
+            if st.op is not None:
+                skeys.append((st.op, st.axes is None, ek, view_of(dst)))
+                continue
+            mk = key_of(st.mask) if st.mask is not None else None
+            if dst.gid in live_gids:
+                dk = ("v", view_of(dst))
+            elif dst.gid in elide:
+                dk = ("e", gid_ids.setdefault(dst.gid, len(gid_ids)), rb_dtype(dst.dtype))
             else:
-                ek = key_of(st[2])
-                skeys.append((st[0], st[1], ek, view_of(st[3])))
+                dk = ("d", gid_ids.setdefault(dst.gid, len(gid_ids)))
+            skeys.append((None, dk, ek, mk))
         if len(views) > cabi.MAX_VIEWS:
             raise ProgramLimit("fused op touches %d array views (max %d)" % (len(views), cabi.MAX_VIEWS))
         if not views or not statements:
@@ -543,8 +499,8 @@ class deferred_op:
         if hit[0] == "limit":
             raise ProgramLimit(hit[1])
         _, prog, gslots, aslots = hit
-        gred = [(slot, statements[si][3]) for (slot, si) in gslots]
-        ared = [(slot, statements[si][3], statements[si][1]) for (slot, si) in aslots]
+        gred = [(slot, statements[si].dst) for (slot, si) in gslots]
+        ared = [(slot, statements[si].dst, statements[si].op) for (slot, si) in aslots]
         return views, prog, gred, ared
 
     def _lower_uncached(self, statements, live_gids, views, vindex, reads):
@@ -557,20 +513,15 @@ class deferred_op:
         lw = Lowering([rb_dtype(det.dtype) for (_, det) in views])
         lw.view_gids = [g for (g, _) in views]
         lw.note_view_reads(reads)
-        temps = {}
         dead_values = {}
 
         def resolve(o):
             if isinstance(o, ArrRef):
-                if o.shape == ():
-                    return lw.scalar(o.value)
                 if o.gid in live_gids:
                     return lw.read_view(view_of(o))
                 if o.gid in dead_values:
                     return dead_values[o.gid]
                 return lw.scalar(0)  # read of an uninitialised, already dead array
-            if isinstance(o, TempVar):
-                return temps[o]
             if isinstance(o, np.ndarray) and o.shape == ():
                 return lw.scalar(o.item())
             return lw.scalar(o)
@@ -578,29 +529,25 @@ class deferred_op:
         gslots = []  # (slot, statement index)
         aslots = []
         for si, st in enumerate(statements):
-            if st[0] == "assign":
-                _, dst, expr, mask = st
-                tv = lw.build(expr, resolve)
-                if isinstance(dst, TempVar):
-                    temps[dst] = tv
-                elif dst.gid in live_gids:
-                    m = resolve(mask) if mask is not None else None
-                    lw.store(view_of(dst), tv, m)
-                elif dst.gid in self.elide_gids:
-                    # an elided temporary keeps the value a store + reload would have given it (the reference
-                    # materialises it: ramba_b200 only skips the memory traffic, not the rounding)
-                    dead_values[dst.gid] = lw.astype(tv, rb_dtype(dst.dtype))
-                else:
-                    if mask is not None and dst.gid in dead_values:
-                        # a masked assignment to an array that lives in a register: elements where the mask is false keep
-                        # the value the array had (`t = a + b; t[m] = 0.5; r = cos(t)` with t never stored)
-                        old = dead_values[dst.gid]
-                        tv = lw.build(E("where", mask, lw.coerce(tv, old.cls), old), resolve)
-                    dead_values[dst.gid] = tv
-            elif st[0] == "gred":
-                gslots.append((lw.reduce(st[1], lw.build(st[2], resolve)), si))
+            tv = lw.build(st.expr, resolve)
+            if st.op is not None:
+                (gslots if st.axes is None else aslots).append((lw.reduce(REDUCTIONS[st.op].code, tv), si))
+                continue
+            dst, mask = st.dst, st.mask
+            if dst.gid in live_gids:
+                m = resolve(mask) if mask is not None else None
+                lw.store(view_of(dst), tv, m)
+            elif dst.gid in self.elide_gids:
+                # an elided temporary keeps the value a store + reload would have given it (the reference
+                # materialises it: ramba_b200 only skips the memory traffic, not the rounding)
+                dead_values[dst.gid] = lw.astype(tv, rb_dtype(dst.dtype))
             else:
-                aslots.append((lw.reduce(st[1], lw.build(st[2], resolve)), si))
+                if mask is not None and dst.gid in dead_values:
+                    # a masked assignment to an array that lives in a register: elements where the mask is false keep
+                    # the value the array had (`t = a + b; t[m] = 0.5; r = cos(t)` with t never stored)
+                    old = dead_values[dst.gid]
+                    tv = lw.build(E("where", mask, lw.coerce(tv, old.cls), old), resolve)
+                dead_values[dst.gid] = tv
         return ("ok", lw.finish(), gslots, aslots)
 
     def _finish(self, live_gids):
@@ -640,8 +587,8 @@ class DAG:
       * while a node executes, API calls made by the executor run inline (`DAG.in_evaluate`), and RAMBA_NO_DAG=1
         makes every call inline."""
 
-    __slots__ = ("seq_no", "expr", "reads", "dst", "out_ref", "write_array", "kw", "shape", "backward_deps", "forward_deps",
-                 "executed", "rgids", "wgids", "__weakref__")
+    __slots__ = ("seq_no", "stmt", "out_ref", "shape", "backward_deps", "forward_deps", "executed", "rgids", "wgid",
+                 "__weakref__")
     pending = {}       # seq_no -> node, in program order
     last_writer = {}   # gid -> pending node that writes the array last
     readers = {}       # gid -> pending nodes that read it since
@@ -652,85 +599,64 @@ class DAG:
     max_pending = 4096
 
     @classmethod
-    def add(cls, oplist, write_array, imports=(), axis_reduce=None, precode=(), postcode=(), elide=None):
-        """Same signature as deferred_op.add_op (the operator seam, ramba/ramba.py:8383-8385)."""
-        if NO_DAG or cls.in_evaluate:
-            deferred_op.add_op(oplist, write_array, imports, axis_reduce, precode, postcode, elide)
-            return
-        dst, expr = oplist[0], oplist[1]
+    def assign(cls, dst, expr):
+        """Defer `dst = expr` (where dst's mask is true)."""
+        cls._add(dst, expr, None, None, None)
+
+    @classmethod
+    def reduce(cls, op, expr, red_view, axes=None, elide=None):
+        """Defer reduction `op` (sum prod min max all any) of expr over `axes` (None: every axis) into the partial array
+        view red_view; `elide`: see deferred_op.add_op."""
+        cls._add(red_view, expr, op, axes, elide)
+
+    @classmethod
+    def _add(cls, dst, expr, op, axes, elide):
+        direct = NO_DAG or cls.in_evaluate
         reads = []
-        _array_operands(expr, reads)
-        if None in reads:
-            expr = _snapshot_0d(expr)
-            reads = [o for o in reads if o is not None]
+        stmt = Statement(dst, _detach(expr, reads, direct), reads, op, axes, elide)
+        if direct:
+            deferred_op.add_op(stmt)
+            return
         node = object.__new__(cls)
         seq = node.seq_no = cls.dag_count
         cls.dag_count = seq + 1
-        node.expr = expr
-        node.reads = reads
-        node.kw = (imports, axis_reduce, precode, postcode, elide)
+        node.stmt = stmt
         node.executed = False
         node.forward_deps = set()
-        dst_nd = isinstance(dst, ndarray)
-        arr = write_array if write_array is not None else (dst if dst_nd else (reads[0] if reads else None))
-        node.shape = arr.shape if arr is not None else None
+        node.shape = dst.shape
         rg = [o.bdarray.gid for o in reads]
-        plain = axis_reduce is None and not precode
-        if write_array is not None:
-            wgid = write_array.bdarray.gid
-            wg = [wgid]
-            if write_array.maskarray is not None:
-                rg.append(write_array.maskarray.gid)
-        else:
-            wgid = None
-            wg = []
-        if dst_nd and dst is not write_array:
-            wg.append(dst.gid)
-        if not plain:
-            if axis_reduce is not None:
-                wg.append(axis_reduce[1].gid)
-            if precode:
-                wg.append(postcode[0].gid)
+        if stmt.mask is not None:
+            rg.append(stmt.mask.gid)
+        wgid = dst.bdarray.gid
         # the destination of an out-of-place statement is the only way to observe it: hold it weakly
-        if plain and dst is write_array and dst_nd and dst.base is None and dst.maskarray is None and wgid not in rg:
-            node.dst = None
-            node.write_array = None
+        if op is None and dst.base is None and stmt.mask is None and wgid not in rg:
+            stmt.dst = None
             node.out_ref = weakref.ref(dst, node._output_died)
         else:
-            node.dst = dst
-            node.write_array = write_array
             node.out_ref = None
         lw, rd = cls.last_writer, cls.readers
         deps = []
         if lw:
-            for g in rg:
-                d = lw.get(g)
-                if d is not None and d not in deps:
-                    deps.append(d)
-            for g in wg:
+            for g in rg + [wgid]:
                 d = lw.get(g)
                 if d is not None and d not in deps:
                     deps.append(d)
         if rd:
-            for g in wg:
-                lst = rd.pop(g, None)
-                if lst:
-                    for d in lst:
-                        if d not in deps:
-                            deps.append(d)
+            for d in rd.pop(wgid, ()):
+                if d not in deps:
+                    deps.append(d)
         for d in deps:
             d.forward_deps.add(node)
         node.backward_deps = deps
         node.rgids = rg
-        node.wgids = wg
+        node.wgid = wgid
         for g in rg:
             lst = rd.get(g)
             if lst is None:
                 rd[g] = [node]
             else:
                 lst.append(node)
-        for g in wg:
-            lw[g] = node
+        lw[wgid] = node
         cls.pending[node.seq_no] = node
         if len(cls.pending) >= cls.max_pending:
             cls.execute_all()
@@ -759,9 +685,8 @@ class DAG:
             except ValueError:
                 pass
         lw, rd = cls.last_writer, cls.readers
-        for g in self.wgids:
-            if lw.get(g) is self:
-                del lw[g]
+        if lw.get(self.wgid) is self:
+            del lw[self.wgid]
         for g in self.rgids:
             lst = rd.get(g)
             if lst is not None:
@@ -778,25 +703,19 @@ class DAG:
         self.backward_deps = ()
         self.forward_deps = ()
         self.out_ref = None
-        self.kw = None
         # last: dropping the operands may end other arrays' lives (and prune their producers through the callback above)
-        self.expr = None
-        self.reads = None
-        self.dst = None
-        self.write_array = None
+        self.stmt = None
 
     def _execute(self):
         """Hand the statement to the fuser (DAG.execute, ramba/ramba.py:4846-4872)."""
-        dst, wa = self.dst, self.write_array
+        stmt = self.stmt
         if self.out_ref is not None:
-            dst = wa = self.out_ref()
-            if dst is None:
+            stmt.dst = self.out_ref()
+            if stmt.dst is None:
                 self._retire(False)  # nobody can observe the result
                 return
-        imports, axis_reduce, precode, postcode, elide = self.kw
-        expr, reads = self.expr, self.reads
         self._retire(True)
-        deferred_op.add_op([dst, expr], wa, imports, axis_reduce, precode, postcode, elide, reads)
+        deferred_op.add_op(stmt)
 
     # ---- materialisation -------------------------------------------------------------------
     @classmethod
@@ -1177,8 +1096,7 @@ class ndarray:
             return False
         return not builtins.any(a > 1 and b > 1 and a != b for a, b in zip(shape[new_dims:], self.shape))
 
-    def array_unaryop(self, op, optext, reduction=False, dtype=None, axis=None, keepdims=False, redop=None, initval=0,
-                      asarray=False, elide=None):
+    def array_unaryop(self, op, optext, reduction=False, dtype=None, axis=None, keepdims=False, asarray=False, elide=None):
         if dtype is None:
             dtype = self.dtype
         elif isinstance(dtype, str) and dtype == "float":
@@ -1186,9 +1104,9 @@ class ndarray:
         dtype = np.dtype(dtype)
         if not reduction:
             new = create_array_with_divisions(self.shape, self.distribution, dtype=dtype)
-            DAG.add([new, E(optext, self)], new)
+            DAG.assign(new, E(optext, self))
             return new
-        return self._reduction(op, redop, dtype, axis, keepdims, initval, asarray, elide)
+        return self._reduction(op, dtype, axis, keepdims, asarray, elide)
 
     def array_binop(self, rhs, op, optext, inplace=False, reverse=False, dtype=None):
         if isinstance(rhs, np.ndarray):
@@ -1215,44 +1133,41 @@ class ndarray:
             if self.readonly:
                 raise ValueError("assignment destination is read-only")
             assert self.shape == new_shape, "non-broadcastable output operand"
-            DAG.add([self, E(optext, self, rhsview)], self)
+            DAG.assign(self, E(optext, self, rhsview))
             return self
         new = empty(new_shape, dtype=new_dtype)
         if reverse:
-            DAG.add([new, E(optext, rhsview, selfview)], new)
+            DAG.assign(new, E(optext, rhsview, selfview))
         else:
-            DAG.add([new, E(optext, selfview, rhsview)], new)
+            DAG.assign(new, E(optext, selfview, rhsview))
         return new
 
     # ---- reductions (ramba/ramba.py:5789-5937)
-    def _reduction(self, op, redop, dtype, axis, keepdims, initval, asarray, elide=None):
+    def _reduction(self, op, dtype, axis, keepdims, asarray, elide=None):
         if axis is not None:
             if isinstance(axis, numbers.Number):
                 axis = [axis]
             axis = sorted(a % self.ndim if -self.ndim <= a < self.ndim else _raise_axis(a, self.ndim) for a in axis)
             if len(axis) == self.ndim:
                 axis = None
-        if isinstance(initval, numbers.Integral) and not isinstance(initval, bool):
-            if initval < 0:
-                initval = getminmax(dtype)[0]
-            elif initval > 1:
-                initval = getminmax(dtype)[1]
+        red = REDUCTIONS[op]
+        init = red.identity(dtype)
+        if red.truth:
+            init = bool(init)  # (the partial array of all / any starts as a truth value)
         if self.maskarray is not None:
             axis = None
         if axis is None or (axis == [0] and self.ndim == 1):
             dsz, dist, bdist = shardview.reduce_all_axes(self.shape, self.distribution)
-            red_arr = full(dsz, initval, dtype=dtype, distribution=dist, no_defer=True)
+            red_arr = full(dsz, init, dtype=dtype, distribution=dist, no_defer=True)
             red_bcast = ndarray(self.shape, base=red_arr, distribution=bdist, local_border=0, readonly=False)
-            tmp = deferred_op.get_temp_var()
-            src = self
-            DAG.add([tmp, self if self.maskarray is None else E("where", self.maskarray, self, red_identity(op, dtype))],
-                               red_bcast, precode=[tmp, initval], postcode=[red_bcast, redop], elide=elide)
+            DAG.reduce(op, self if self.maskarray is None else E("where", self.maskarray, self, red_identity(op, dtype)),
+                       red_bcast, elide=elide)
             return _reduction2b(red_arr, op, dtype, asarray)
         dsz, dist, bdist = shardview.reduce_axes(self.shape, self.distribution, axis)
-        red_arr = full(dsz, initval, dtype=dtype, distribution=dist, no_defer=True)
+        red_arr = full(dsz, init, dtype=dtype, distribution=dist, no_defer=True)
         red_bcast = ndarray(self.shape, base=red_arr, distribution=bdist, local_border=0, readonly=False)
-        DAG.add([red_bcast, self], red_bcast, axis_reduce=(axis, red_bcast), postcode=[red_bcast, redop], elide=elide)
-        return _reduction2(red_arr, op, redop, dtype, axis, keepdims is True)
+        DAG.reduce(op, self, red_bcast, axis, elide)
+        return _reduction2(red_arr, op, dtype, axis, keepdims is True)
 
     def mean(self, axis=None, dtype=None, **kwargs):
         n = self.size if axis is None else int(np.prod([self.shape[a] for a in ([axis] if isinstance(axis, numbers.Number) else axis)]))
@@ -1368,19 +1283,19 @@ class ndarray:
             if value.size == 1:
                 value = value.reshape(())
         if isinstance(value, (numbers.Number, np.generic)) or (isinstance(value, np.ndarray) and value.shape == ()):
-            DAG.add([view, value if not isinstance(value, np.ndarray) else value.item()], view)
+            DAG.assign(view, value if not isinstance(value, np.ndarray) else value.item())
             return
         if isinstance(value, np.ndarray):
             value = fromarray(value)
         if value.shape == ():
-            DAG.add([view, value.distribution.item()], view)
+            DAG.assign(view, value.distribution.item())
             return
         if not value.broadcastable_to(view.shape):
             raise ValueError("could not broadcast input array from shape %s into shape %s" % (value.shape, view.shape))
         if value.shape != view.shape:
             value = value.broadcast_to(view.shape)
         if not (view.gid == value.gid and shardview.dist_is_eq(view.distribution, value.distribution)):
-            DAG.add([view, value], view)
+            DAG.assign(view, value)
 
     def remapped_axis(self, newmap):
         if self.bdarray.flex_dist or not self.bdarray.remote_constructed:
@@ -1459,12 +1374,12 @@ class ndarray:
         if dtype == self.dtype:
             return globals()["copy"](self) if copy else self
         new = create_array_with_divisions(self.shape, self.distribution, dtype=dtype)
-        DAG.add([new, self], new)
+        DAG.assign(new, self)
         return new
 
     def clip(self, a_min, a_max, out=None):
         new = out if out is not None else create_array_with_divisions(self.shape, self.distribution, dtype=self.dtype)
-        DAG.add([new, E("min", a_max, E("max", self, a_min))], new)
+        DAG.assign(new, E("min", a_max, E("max", self, a_min)))
         return new
 
     def allclose(self, other, rtol=1e-5, atol=1e-8, equal_nan=False):
@@ -1538,10 +1453,6 @@ def _raise_axis(a, nd):
     raise np.exceptions.AxisError(a, nd)
 
 
-def _np_reduce(op):
-    return {"sum": np.sum, "prod": np.prod, "min": np.min, "max": np.max, "all": np.all, "any": np.any}[op]
-
-
 def _local_partial_tensor(red_arr, n, op):
     """This rank's block of the partial array as a flat device tensor of n elements in the accumulator dtype (float64 /
     int64) - the reduction's identity when the rank holds no part."""
@@ -1570,11 +1481,11 @@ def _reduction2b(red_arr, op, dtype, asarray):
         t = _local_partial_tensor(red_arr, 1, op)
         RT.all_reduce(t, op)
         val = t.cpu().numpy()[0]
-        if op in ("all", "any"):
+        if REDUCTIONS[op].truth:
             val = np.bool_(val != 0)
     else:
         local = np.array(red_arr.asarray())
-        val = _np_reduce(op)(local)
+        val = getattr(np, op)(local)  # (NumPy names its reductions the same)
     if not asarray:
         return np.sum(val, dtype=dtype)
     return full((1,), val, dtype=dtype)
@@ -1595,7 +1506,7 @@ def _split_only_along(red_arr, axis):
     return True
 
 
-def _reduction2(red_arr, op, redop, dtype, axis, keepdims):
+def _reduction2(red_arr, op, dtype, axis, keepdims):
     """Stage 2 of an axis reduction: fold the per-division partial slices (ramba/ramba.py:5818-5849).  When the
     partial rows live on different ranks and each rank holds whole rows, they are summed by ONE all-reduce (each rank
     then keeps its own division of the result); otherwise a second fused op over the partial slices does it."""
@@ -1609,7 +1520,7 @@ def _reduction2(red_arr, op, redop, dtype, axis, keepdims):
     if builtins.all(x == 1 for x in k):
         return red_arr if keepdims else red_arr[sl1]
     kept_elems = int(np.prod([red_arr.shape[d] for d in range(nd) if d not in axis]))
-    if common.num_workers > 1 and op in ALLREDUCE_OP and kept_elems <= (1 << 24) and _split_only_along(red_arr, axis):
+    if common.num_workers > 1 and kept_elems <= (1 << 24) and _split_only_along(red_arr, axis):
         DAG.instantiate(red_arr)
         w = common.worker_num
         t = _local_partial_tensor(red_arr, kept_elems, op)
@@ -1623,7 +1534,7 @@ def _reduction2(red_arr, op, redop, dtype, axis, keepdims):
             sh.interior().copy_(mine)  # (converts the accumulator dtype back to the array's)
         return arr if keepdims else arr[sl1]
     arr = empty_like(red_arr[sl2])
-    name = {cabi.RED_ADD: "add", cabi.RED_MUL: "mul", cabi.RED_MIN: "min", cabi.RED_MAX: "max"}[redop]
+    combine = REDUCTIONS[op].combine
     expr = None
     for j in np.ndindex(tuple(k)):
         sl = []
@@ -1635,8 +1546,8 @@ def _reduction2(red_arr, op, redop, dtype, axis, keepdims):
             else:
                 sl.append(slice(None))
         piece = red_arr[tuple(sl)]
-        expr = piece if expr is None else E(name, expr, piece)
-    DAG.add([arr, expr], arr)
+        expr = piece if expr is None else E(combine, expr, piece)
+    DAG.assign(arr, expr)
     return arr[sl1]
 
 
@@ -1716,7 +1627,7 @@ for _n, (_t, _d) in array_unaryop_funcs.items():
     setattr(ndarray, _n, _make_unop(_n, _t, dtype=_d))
 
 
-def _make_reduction(name, redop, init, dtype=None):
+def _make_reduction(name, dtype=None):
     def _method(self, axis=None, dtype=dtype, keepdims=False, asarray=False, **kwargs):
         # `(X*2.0 + 1.0).sum()`: the operand is a temporary that nobody can observe once this call returns.  The global
         # reduction flushes INSIDE the call, while the caller's expression still holds the temporary, so the reference
@@ -1726,8 +1637,8 @@ def _make_reduction(name, redop, init, dtype=None):
         if _sys_getrefcount(self) <= _TEMP_REFCOUNT and self.base is None and self.bdarray.nrefs == 1 \
                 and not self.bdarray.remote_constructed:
             elide = self.gid  # (add_op honours it only if the statement writing the temporary shares the fused op)
-        return self.array_unaryop(name, None, reduction=True, dtype=dtype, axis=axis, keepdims=keepdims, redop=redop,
-                                  initval=init, asarray=asarray, elide=elide)
+        return self.array_unaryop(name, None, reduction=True, dtype=dtype, axis=axis, keepdims=keepdims, asarray=asarray,
+                                  elide=elide)
 
     _method.__name__ = name
     return _method
@@ -1756,12 +1667,9 @@ def _measure_temp_refcount():
 _TEMP_REFCOUNT = _measure_temp_refcount()
 
 
-array_simple_reductions = {
-    "sum": (cabi.RED_ADD, 0, None), "prod": (cabi.RED_MUL, 1, None), "min": (cabi.RED_MIN, 2, None),
-    "max": (cabi.RED_MAX, -2, None), "all": (cabi.RED_MUL, True, np.bool_), "any": (cabi.RED_ADD, False, np.bool_),
-}
-for _n, (_r, _i, _d) in array_simple_reductions.items():
-    setattr(ndarray, _n, _make_reduction(_n, _r, _i, _d))
+array_simple_reductions = {"sum": None, "prod": None, "min": None, "max": None, "all": np.bool_, "any": np.bool_}  # -> default dtype
+for _n, _d in array_simple_reductions.items():
+    setattr(ndarray, _n, _make_reduction(_n, _d))
 
 
 # =============================================================================================
@@ -1982,7 +1890,7 @@ def create_array(shape, filler, local_border=0, dtype=None, distribution=None, n
         # the producers of a reduction stay fused with it (ramba/ramba.py:5918, 8603-8627)
         _fill_now(new, filler)
         return new
-    DAG.add([new, filler], new)
+    DAG.assign(new, filler)
     return new
 
 
@@ -2059,7 +1967,7 @@ def full_like(other, v, dtype=None, **kwargs):
 
 def copy(arr, local_border=0):
     new = create_array_with_divisions(arr.shape, arr.distribution, dtype=arr.dtype)
-    DAG.add([new, arr], new)
+    DAG.assign(new, arr)
     return new
 
 
@@ -2078,7 +1986,7 @@ def arange(start, stop=None, step=None, dtype=None, *, like=None, local_border=0
         expr = E("add", start, Iota(0))
     else:
         expr = E("add", start, E("mul", step, Iota(0)))
-    DAG.add([res, expr], res)
+    DAG.assign(res, expr)
     return res
 
 
@@ -2102,7 +2010,7 @@ def fromfunction(function, shape, dtype=None, **kwargs):
     idx = []
     for d in range(len(shape)):
         a = empty(shape, dtype=np.int64)
-        DAG.add([a, Iota(d)], a)
+        DAG.assign(a, Iota(d))
         idx.append(a)
     out = function(*idx)
     if not isinstance(out, ndarray):
@@ -2229,7 +2137,7 @@ def where(cond, a=None, b=None):
 
     adt = a.dtype if isinstance(a, ndarray) else np.asarray(a).dtype
     new = empty(shape, dtype=adt)
-    DAG.add([new, E("where", view(cond), view(a), view(b))], new)
+    DAG.assign(new, E("where", view(cond), view(a), view(b)))
     return new
 
 
@@ -2459,7 +2367,7 @@ def sstencil(func, *args, out=None, **kwargs):
         # like the reference: allocated with the divisions and the border of the first argument (ramba/ramba.py:10022-10026)
         new = create_array_with_divisions(shape, arrays[0].distribution, local_border=arrays[0].local_border,
                                           dtype=res.dtype if isinstance(res, ndarray) else np.float64)
-        DAG.add([new, 0], new)
+        DAG.assign(new, 0)
     else:
         new = zeros(shape, dtype=res.dtype if isinstance(res, ndarray) else np.float64)
     interior = tuple(slice(-lo[d], shape[d] - hi[d]) for d in range(k))
@@ -2721,7 +2629,7 @@ def _index_arrays(shape):
     idx = []
     for d in range(len(shape)):
         a = empty(shape, dtype=np.int64)
-        DAG.add([a, Iota(d)], a)
+        DAG.assign(a, Iota(d))
         idx.append(a)
     return idx
 
@@ -2805,7 +2713,7 @@ def sreduce_index(func, reducer, identity, *args, parallel=True):
     return _sreduce("sreduce_index", func, reducer, identity, args, True)
 
 
-def _scan_native(a, axis, op, dtype):
+def _scan_native(a, axis, kind, dtype):
     """cumsum / cumprod / running min / max along `axis` with the single-pass scan kernel (rb200_cumulative): every
     rank scans its own block; when the array is cut along the scan axis the block totals are all-gathered and every rank
     folds the totals of the blocks before its own into its part (the reference passes boundary values worker to worker,
@@ -2840,14 +2748,15 @@ def _scan_native(a, axis, op, dtype):
     length = int(lshape[axis]) if not mine_empty else 0
     n_inner = int(np.prod(lshape[axis + 1:])) if not mine_empty else 1
     code = rb_dtype(out_dtype)
+    red = REDUCTIONS[kind]
     acc_dt = torch.float64 if out_dtype.kind == "f" else torch.int64
     ncols = int(np.prod([src.shape[d] for d in range(nd) if d != axis]))
     totals = torch.empty(max(1, ncols), dtype=acc_dt, device=RT.device) if split_axis else None
     if totals is not None:
-        totals.fill_(red_identity({cabi.RED_ADD: "sum", cabi.RED_MUL: "prod", cabi.RED_MIN: "min", cabi.RED_MAX: "max"}[op], out_dtype))
+        totals.fill_(red.identity(out_dtype))
     scratch = carry = None
     if not mine_empty:
-        scratch = RT.cumulative(sh_src.ptr(0), sh_res.ptr(0), code, n_outer, length, n_inner, op, None, totals.data_ptr() if totals is not None else None)
+        scratch = RT.cumulative(sh_src.ptr(0), sh_res.ptr(0), code, n_outer, length, n_inner, red.code, None, totals.data_ptr() if totals is not None else None)
     if split_axis and W > 1:
         allt = torch.empty(W * ncols, dtype=acc_dt, device=RT.device)
         RT.all_gather(allt, totals).wait()
@@ -2855,11 +2764,10 @@ def _scan_native(a, axis, op, dtype):
             before = [p for p in range(W) if not shardview.is_empty(dist[p]) and int(dist[p].start[axis]) < int(dist[w].start[axis])]
             if before:
                 stack = allt.view(W, ncols)[before]
-                carry = {cabi.RED_ADD: stack.sum(0), cabi.RED_MUL: stack.prod(0), cabi.RED_MIN: stack.min(0).values, cabi.RED_MAX: stack.max(0).values}[op]
-                carry = carry.contiguous()
+                carry = red.fold(stack).contiguous()
                 acc_code = cabi.F64 if acc_dt == torch.float64 else cabi.I64
                 # res[o, l, i] = carry[o, i] (op) res[o, l, i] for every l: one fused op with the carry broadcast along the axis
-                RT.launch(_combine_program(code, acc_code, op), [n_outer, length, n_inner], [0, 0, 0],
+                RT.launch(_combine_program(code, acc_code, red.combine), [n_outer, length, n_inner], [0, 0, 0],
                           [(sh_res.ptr(0), [length * n_inner, n_inner, 1], code, sh_res.bounds), (carry.data_ptr(), [n_inner, 0, 1], acc_code)])
     RT.hold(scratch, carry)  # (read only by the launches above)
     return res
@@ -2880,19 +2788,24 @@ def scumulative(local_func, final_func, array, axis=None, dtype=None, out=None):
         kind = _classify_reducer(f)
     except NotImplementedError:
         kind = None
-    if kind is not None and array.size > 0:
-        op = {"sum": cabi.RED_ADD, "prod": cabi.RED_MUL, "min": cabi.RED_MIN, "max": cabi.RED_MAX}[kind]
-        res = _scan_native(array, int(axis), op, dtype)
+    return _scan(array, int(axis), kind, f, dtype)
+
+
+def _scan(a, axis, kind, step, dtype):
+    """Inclusive scan of `a` along `axis`: reduction `kind` on the scan kernel when it covers the layout, otherwise (or
+    when kind is None) log2(n) fused shifted-slice steps `hi = step(lo, hi)`."""
+    if kind is not None and a.size > 0:
+        res = _scan_native(a, axis, kind, dtype)
         if res is not None:
             return res
-    cur = array.astype(dtype) if dtype is not None and np.dtype(dtype) != array.dtype else array + 0
-    n = array.shape[axis]
+    cur = a.astype(dtype) if dtype is not None and np.dtype(dtype) != a.dtype else a + 0
+    n = a.shape[axis]
     d = 1
     while d < n:
-        nxt = cur + 0
-        hi = tuple(slice(d, None) if k == axis else slice(None) for k in range(array.ndim))
-        lo = tuple(slice(0, n - d) if k == axis else slice(None) for k in range(array.ndim))
-        nxt[hi] = f(cur[lo], cur[hi])
+        nxt = cur + 0  # fresh array: a step reads the previous one at two offsets, it cannot run in place
+        hi = tuple(slice(d, None) if k == axis else slice(None) for k in range(a.ndim))
+        lo = tuple(slice(0, n - d) if k == axis else slice(None) for k in range(a.ndim))
+        nxt[hi] = step(cur[lo], cur[hi])
         cur = nxt
         d *= 2
     return cur
@@ -2910,21 +2823,7 @@ def cumsum(a, axis=None, dtype=None, out=None):
         axis = 0
     assert isinstance(axis, numbers.Number) and 0 <= axis < a.ndim, "cumsum needs an axis for N-d arrays"
     assert out is None, "cumsum(out=...) is not supported (nor by the reference, ramba/ramba.py:10071-10075)"
-    if a.size > 0:
-        res = _scan_native(a, int(axis), cabi.RED_ADD, dtype)
-        if res is not None:
-            return res
-    cur = a.astype(dtype) if dtype is not None and np.dtype(dtype) != a.dtype else a + 0
-    n = a.shape[axis]
-    d = 1
-    while d < n:
-        nxt = cur + 0  # fresh array: a step reads the previous one at two offsets, it cannot run in place
-        hi = tuple(slice(d, None) if k == axis else slice(None) for k in range(a.ndim))
-        lo = tuple(slice(0, n - d) if k == axis else slice(None) for k in range(a.ndim))
-        nxt[hi] = cur[hi] + cur[lo]
-        cur = nxt
-        d *= 2
-    return cur
+    return _scan(a, int(axis), "sum", lambda lo, hi: hi + lo, dtype)
 
 
 def instantiate_all(*args, **kwargs):

@@ -118,7 +118,7 @@ class _State:
         expr = E("philox", *args, imm=form)
         if tail is not None:
             expr = tail(expr)
-        _r.DAG.add([res, expr], res)
+        _r.DAG.assign(res, expr)
         return res
 
     # ---- the distributions

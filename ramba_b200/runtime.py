@@ -23,7 +23,7 @@ import torch.distributed as dist
 from . import _cabi as cabi
 from . import common
 from . import shardview
-from .program import np_dtype, rb_dtype
+from .program import REDUCTIONS, np_dtype, rb_dtype
 
 _TORCH_DTYPE = {
     np.dtype(np.float64): torch.float64,
@@ -41,10 +41,6 @@ _TORCH_DTYPE = {
 
 def torch_dtype(dt):
     return _TORCH_DTYPE[np.dtype(dt)]
-
-
-# reductions an all-reduce can combine, and how (all / any of 0/1 values are min / max)
-ALLREDUCE_OP = {"sum": "SUM", "prod": "PRODUCT", "min": "MIN", "max": "MAX", "all": "MIN", "any": "MAX"}
 
 
 class Shard:
@@ -244,7 +240,7 @@ class Runtime:
         self.ensure_process_group()
         self.collectives += 1
         self.bytes_sent += t.numel() * t.element_size()
-        dist.all_reduce(t, op=getattr(dist.ReduceOp, ALLREDUCE_OP[op]))
+        dist.all_reduce(t, op=getattr(dist.ReduceOp, REDUCTIONS[op].allreduce))
 
     def broadcast(self, t, src):
         """Rank src's t into every rank's t, in place."""

@@ -34,15 +34,15 @@ def _captured_programs(monkeypatch):
     progs = []
     orig = ramba.run_deferred_ops
 
-    def spy(uuid, views, prog, *args, **kwargs):
+    def spy(views, prog, *args, **kwargs):
         progs.append(prog)
-        return orig(uuid, views, prog, *args, **kwargs)
+        return orig(views, prog, *args, **kwargs)
 
     monkeypatch.setattr(ramba, "run_deferred_ops", spy)
     return progs
 
 
-def test_fusion_like_the_reference(oracle_engine, monkeypatch):
+def test_fusion_counts_like_the_reference(oracle_engine, monkeypatch):
     """TestFusion (ramba/tests/test_distributed_array.py:112-198): ten `a += 1` between two syncs are ONE
     fused op that reads and writes `a` once; ten `a[i:] += 1` cannot fuse (ten flushes); an expression with
     several temporaries materialises none of them."""
