@@ -63,8 +63,11 @@ def shapeToInt(shape):
 # bdarray: the physical distributed buffer
 # =============================================================================================
 class bdarray:
-    gid_map = weakref.WeakValueDictionary()
-    __slots__ = ("shape", "gid", "pad", "distribution", "nrefs", "remote_constructed", "flex_dist", "dtype", "failed", "__weakref__")
+    """remote_constructed: the array's blocks exist (a flush or blocks.block made them).  flex_dist: its partition can
+    still be pinned to that of the fused op it is used in.  Whatever sets remote_constructed clears flex_dist, so
+    flex_dist implies not remote_constructed."""
+
+    __slots__ = ("shape", "gid", "pad", "distribution", "nrefs", "remote_constructed", "flex_dist", "dtype", "failed")
 
     def __init__(self, shape, distribution, gid, pad, fdist, dtype):
         self.shape = shape
@@ -76,7 +79,6 @@ class bdarray:
         self.flex_dist = fdist
         self.dtype = np.dtype(dtype)
         self.failed = None  # why the last fused op that wrote this array did not run (its contents are undefined then)
-        bdarray.gid_map[gid] = self
 
     def ndarray_del_callback(self):
         self.nrefs -= 1
@@ -84,10 +86,9 @@ class bdarray:
             deferred_op.del_remote_array(self.gid)
 
     @classmethod
-    def assign_bdarray(cls, nd, shape, gid=None, distribution=None, pad=0, flexible_dist=False, dtype=None, **kwargs):
-        if gid is None:
-            gid = _new_gid()
-        bd = cls.gid_map.get(gid)
+    def assign_bdarray(cls, nd, shape, base=None, distribution=None, pad=0, flexible_dist=False, dtype=None, **kwargs):
+        """The buffer of a new handle: `base`'s (a bdarray) for a view, else a new one."""
+        bd = base
         if bd is None:
             if dtype is None:
                 dtype = np.float64
@@ -98,17 +99,9 @@ class bdarray:
             else:
                 # a new array: same boxes, fresh buffer coordinates
                 distribution = shardview.clean_dist(distribution)
-            bd = cls(shape, distribution, gid, pad, flexible_dist, dtype)
+            bd = cls(shape, distribution, _new_gid(), pad, flexible_dist, dtype)
         bd.nrefs += 1
         return bd
-
-    @classmethod
-    def get_by_gid(cls, gid):
-        return cls.gid_map[gid]
-
-    @classmethod
-    def valid_gid(cls, gid):
-        return gid in cls.gid_map
 
 
 class ndarray_details:
@@ -181,6 +174,14 @@ class Statement:
         self.op, self.axes, self.elide = op, axes, elide
 
 
+def _other_view(dists, dist):
+    """True when one of `dists` (None: a partition that was still flexible) is not `dist`."""
+    for d in dists:
+        if d is not None and not shardview.dist_is_eq(d, dist):
+            return True
+    return False
+
+
 def _walk_operands(x, out):
     if isinstance(x, E):
         for a in x.args:
@@ -207,6 +208,24 @@ def _check_same_lowering(a, b):
         raise AssertionError("lowering memo returned a different op list for the same structural key")
 
 
+class _Use:
+    """What the pending fused op knows about one array its statements touch.
+      bd        the array's bdarray, held until the flush pins its partition and marks its blocks made
+      reads     the distributions statements read the array through (None where its partition was still flexible)
+      writes    the same for the statements that store into it
+      flexible  its partition was flexible at its first admission: the flush pins it to the op's
+      resident  its blocks existed at an admission: the flush keeps it in memory even if every handle has died"""
+
+    __slots__ = ("bd", "reads", "writes", "flexible", "resident")
+
+    def __init__(self, bd):
+        self.bd = bd
+        self.reads = []
+        self.writes = []
+        self.flexible = bd.flex_dist
+        self.resident = False
+
+
 class deferred_op:
     ramba_deferred_ops = None
     max_statements = 40
@@ -215,32 +234,21 @@ class deferred_op:
         self.shape = shape
         self.distribution = distribution
         self.flex_dist = fdist
-        self.delete_gids = []
-        self.read_arrs = []
-        self.write_arrs = []
-        self.read_gids = set()   # (gids of read_arrs / write_arrs: the alias checks look at the lists only on a gid match)
-        self.write_gids = set()
-        self.use_gids = {}  # gid -> ([(view index within gid, details)], bd_shape, bd_distribution, pad, flex)
-        self.preconstructed_gids = {}
+        self.arrays = {}    # gid -> _Use, for every array a statement of this op reads, stores or reduces into
+        self.dead = set()   # arrays whose last handle died while this op was pending
+        self.elide = set()  # arrays proven unobservable after the flush (dying temporaries of a reduction)
         self.statements = []
         self.red_axes = None  # the axes every axis reduction of this op reduces over (ramba/ramba.py:8425-8432)
-        self.keepalives = set()
-        self.elide_gids = set()  # arrays proven unobservable after the flush (dying temporaries of a reduction)
 
-    def add_gid(self, nd):
-        gid = nd.bdarray.gid
-        ent = self.use_gids.get(gid)
-        if ent is None:
-            bd = nd.bdarray
-            ent = self.use_gids[gid] = ([], bd.shape, bd.distribution, bd.pad, bd.flex_dist and not bd.remote_constructed)
-            self.keepalives.add(bd)
-        ndist = nd.distribution
-        for det in ent[0]:
-            if det.distribution is ndist or shardview.dist_is_eq(det.distribution, ndist):
-                return
-        ent[0].append(_ref_of(nd))
-        if nd.bdarray.remote_constructed:
-            self.preconstructed_gids[gid] = True
+    def _use(self, nd):
+        """The record of nd's array, made at its first admission; marks it resident when its blocks exist now."""
+        bd = nd.bdarray
+        u = self.arrays.get(bd.gid)
+        if u is None:
+            u = self.arrays[bd.gid] = _Use(bd)
+        if bd.remote_constructed:
+            u.resident = True
+        return u
 
     # ---- adding statements --------------------------------------------------------------
     @classmethod
@@ -259,7 +267,7 @@ class deferred_op:
         abd = dst.bdarray
         # the partition of `dst` can still follow the op's only if dst is a whole array that no flush has touched: a VIEW of
         # a flexible array was cut from the partition the array had then and does not move when the array is pinned
-        fixed = abd.remote_constructed or not abd.flex_dist or dst.base is not None
+        fixed = not abd.flex_dist or dst.base is not None
         cur = cls.ramba_deferred_ops
         if cur is not None:
             if (cur.shape != shape
@@ -273,34 +281,23 @@ class deferred_op:
                 cls.do_ops()
                 cur = None
         # alias check 1: reads/writes a shifted version of an array written earlier in this op
-        if cur is not None and cur.write_gids:
-            wg = cur.write_gids
-            hit = False
+        if cur is not None:
             for o in operands:
-                if o.bdarray.gid in wg:
-                    og, od = o.bdarray.gid, o.distribution
-                    for (wgid, wdist) in cur.write_arrs:
-                        if wgid == og and wdist is not None and not shardview.dist_is_eq(wdist, od):
-                            hit = True
-                            break
-                    if hit:
-                        break
-            if hit:
-                cls.do_ops()
-                cur = None
+                u = cur.arrays.get(o.gid)
+                if u is not None and _other_view(u.writes, o.distribution):
+                    cls.do_ops()
+                    cur = None
+                    break
         # alias check 2: writes an array that is also read through a different view
         if stores:
-            wgid, wdist = abd.gid, dst.distribution
             hit = False
             for o in operands:
-                if o is not dst and o.bdarray.gid == wgid and not shardview.dist_is_eq(o.distribution, wdist):
+                if o is not dst and o.gid == abd.gid and not shardview.dist_is_eq(o.distribution, distribution):
                     hit = True
                     break
-            if not hit and cur is not None and wgid in cur.read_gids:
-                for (rgid, rdist) in cur.read_arrs:
-                    if rgid == wgid and rdist is not None and not shardview.dist_is_eq(rdist, wdist):
-                        hit = True
-                        break
+            if not hit and cur is not None:
+                u = cur.arrays.get(abd.gid)
+                hit = u is not None and _other_view(u.reads, distribution)
             if hit:
                 tmp_array = empty_like(dst)
                 cls.add_op(Statement(tmp_array, stmt.expr, reads))
@@ -312,27 +309,23 @@ class deferred_op:
         if fixed and (cur.flex_dist or not abd.flex_dist):
             cur.distribution = distribution
             cur.flex_dist = False
-        elide = stmt.elide
-        if elide is not None and elide in cur.write_gids and bdarray.valid_gid(elide) \
-                and not bdarray.get_by_gid(elide).remote_constructed:
+        u = cur.arrays.get(stmt.elide) if stmt.elide is not None else None
+        if u is not None and u.writes and not u.bd.remote_constructed:
             # (decided HERE, after admission: a flush forced by this very statement must still materialise the operand)
-            cur.elide_gids.add(elide)
+            cur.elide.add(stmt.elide)
         mask = stmt.mask
         if stores:
             if mask is not None:
                 operands = [mask] + operands
-            cur.write_arrs.append((abd.gid, None if abd.flex_dist else distribution))
-            cur.write_gids.add(abd.gid)
-        read_arrs, read_gids = cur.read_arrs, cur.read_gids
+            if dst.shape != ():  # (like the operand list above, the op keeps no record of a 0-d destination)
+                cur._use(dst).writes.append(None if abd.flex_dist else distribution)
         for x in operands:
             xbd = x.bdarray
             if xbd.failed is not None:
                 _raise_failed(xbd)
-            read_arrs.append((xbd.gid, None if xbd.flex_dist else x.distribution))
-            read_gids.add(xbd.gid)
-            cur.add_gid(x)
+            cur._use(x).reads.append(None if xbd.flex_dist else x.distribution)
         if stmt.op is not None:
-            cur.add_gid(dst)
+            cur._use(dst)
             if stmt.axes is not None:
                 cur.red_axes = stmt.axes
         stmt.dst = _ref_of(dst)
@@ -346,7 +339,7 @@ class deferred_op:
         if cls.ramba_deferred_ops is None:
             RT.destroy_array(gid)
         else:
-            cls.ramba_deferred_ops.delete_gids.append(gid)
+            cls.ramba_deferred_ops.dead.add(gid)
 
     @classmethod
     def do_ops(cls):
@@ -357,57 +350,56 @@ class deferred_op:
 
     # ---- flush ---------------------------------------------------------------------------
     def execute(self):
+        """Run the op.  An array lives in memory if its blocks existed at an admission or someone can still read it after
+        the flush; every other array is a register temporary."""
         t0 = timer()
-        live_gids = {
-            k: v for (k, v) in self.use_gids.items()
-            if (bdarray.valid_gid(k) and k not in self.delete_gids and k not in self.elide_gids) or k in self.preconstructed_gids
-        }
-        self._pin(live_gids)
+        dead, elide = self.dead, self.elide
+        live = {g for (g, u) in self.arrays.items() if u.resident or (g not in dead and g not in elide)}
+        self._pin(live)
         try:
-            self._run_statements(self.statements, live_gids)
+            self._run_statements(self.statements, live)
         except BaseException as ex:
             # the statements of this op are gone: what they were to write is undefined from here on.  Reading it later must
             # fail loudly, not return whatever the shard holds (the reference re-raises on the driver and stops there,
             # ramba/ramba.py:3875-3881, 4053-4054)
             why = "%s: %s" % (type(ex).__name__, str(ex)[:300])
-            for g in self.write_gids:
-                bd = bdarray.gid_map.get(g)
-                if bd is not None:
-                    bd.failed = why
+            for u in self.arrays.values():
+                if u.writes:
+                    u.bd.failed = why
             raise
         finally:
-            self._finish(live_gids)
+            self._finish(live)
         add_time("driver_deferred_op", timer() - t0)
 
     def _pin(self, gids):
         """Pin flexible distributions to the op's distribution (ramba/ramba.py:8130-8136)."""
-        for (_, (_, s, d, _, flex)) in gids.items():
-            if flex and self.shape == s:
-                d[:] = shardview.clean_dist(self.distribution)
+        for g in gids:
+            u = self.arrays[g]
+            if u.flexible and u.bd.shape == self.shape:
+                u.bd.distribution[:] = shardview.clean_dist(self.distribution)
 
-    def _run_statements(self, statements, live_gids):
+    def _run_statements(self, statements, live):
         """Lower `statements` to one op list and launch it.  The reference never fails on the length of a fused chain
         (Numba compiles whatever the fuser accumulated); a prebuilt library has table sizes (views, spill registers,
         instructions, scalars, reduction slots), so a chain that exceeds one of them is cut in two at a statement
         boundary and run as two launches: arrays that are written before the cut and read after it, and would
         otherwise have stayed register temporaries, are materialised for the duration of the flush."""
         try:
-            lowered = self._lower(statements, live_gids)
+            lowered = self._lower(statements, live)
         except ProgramLimit:
             if len(statements) < 2:
                 raise
             m = len(statements) // 2
             first, second = statements[:m], statements[m:]
             written = {st.dst.gid for st in first if st.op is None}
-            crossing = {}
+            crossing = set()
             for st in second:
                 for x in (st.expr, st.mask):
                     for o in _walk_operands(x, []):
-                        if isinstance(o, ArrRef) and o.gid in written and o.gid not in live_gids:
-                            crossing[o.gid] = self.use_gids[o.gid]
+                        if isinstance(o, ArrRef) and o.gid in written and o.gid not in live:
+                            crossing.add(o.gid)
             self._pin(crossing)
-            both = dict(live_gids)
-            both.update(crossing)
+            both = live | crossing
             try:
                 self._run_statements(first, both)
                 self._run_statements(second, both)
@@ -424,7 +416,7 @@ class deferred_op:
         run_deferred_ops(views, prog, self.distribution, gred, ared, self.red_axes if ared else None)
         add_time("run_deferred_ops", timer() - t1)
 
-    def _lower(self, statements, live_gids):
+    def _lower(self, statements, live):
         """Statements -> (view table, op list, global reductions, axis reductions).  The op list depends only on the
         STRUCTURE of the statements (operators, which operand is which view / temporary / dead array, view dtypes and
         aliasing, scalar values), not on the arrays themselves, so it is memoised on that structure: the second and
@@ -434,7 +426,7 @@ class deferred_op:
         vindex = {}
         reads = {}
         gid_ids = {}
-        elide = self.elide_gids
+        elide = self.elide
 
         def view_of(nd):
             lst = vindex.setdefault(nd.gid, [])
@@ -451,7 +443,7 @@ class deferred_op:
             if isinstance(x, E):
                 return (x.op, x.imm) + tuple([key_of(a) for a in x.args])
             if isinstance(x, ArrRef):
-                if x.gid in live_gids:
+                if x.gid in live:
                     i = view_of(x)
                     reads[i] = reads.get(i, 0) + 1
                     return ("v", i)
@@ -470,7 +462,7 @@ class deferred_op:
                 skeys.append((st.op, st.axes is None, ek, view_of(dst)))
                 continue
             mk = key_of(st.mask) if st.mask is not None else None
-            if dst.gid in live_gids:
+            if dst.gid in live:
                 dk = ("v", view_of(dst))
             elif dst.gid in elide:
                 dk = ("e", gid_ids.setdefault(dst.gid, len(gid_ids)), rb_dtype(dst.dtype))
@@ -487,7 +479,7 @@ class deferred_op:
         hit = _lower_cache.get(key)
         if hit is None or _VERIFY_LOWER_CACHE:
             try:
-                fresh = self._lower_uncached(statements, live_gids, views, vindex, reads)
+                fresh = self._lower_uncached(statements, live, views, vindex, reads)
             except ProgramLimit as e:
                 fresh = ("limit", str(e))
             if hit is not None:
@@ -503,7 +495,7 @@ class deferred_op:
         ared = [(slot, statements[si].dst, statements[si].op) for (slot, si) in aslots]
         return views, prog, gred, ared
 
-    def _lower_uncached(self, statements, live_gids, views, vindex, reads):
+    def _lower_uncached(self, statements, live, views, vindex, reads):
         def view_of(nd):
             for (dist, idx) in vindex[nd.gid]:
                 if dist is nd.distribution or shardview.dist_is_eq(dist, nd.distribution):
@@ -517,7 +509,7 @@ class deferred_op:
 
         def resolve(o):
             if isinstance(o, ArrRef):
-                if o.gid in live_gids:
+                if o.gid in live:
                     return lw.read_view(view_of(o))
                 if o.gid in dead_values:
                     return dead_values[o.gid]
@@ -534,10 +526,10 @@ class deferred_op:
                 (gslots if st.axes is None else aslots).append((lw.reduce(REDUCTIONS[st.op].code, tv), si))
                 continue
             dst, mask = st.dst, st.mask
-            if dst.gid in live_gids:
+            if dst.gid in live:
                 m = resolve(mask) if mask is not None else None
                 lw.store(view_of(dst), tv, m)
-            elif dst.gid in self.elide_gids:
+            elif dst.gid in self.elide:
                 # an elided temporary keeps the value a store + reload would have given it (the reference
                 # materialises it: ramba_b200 only skips the memory traffic, not the rounding)
                 dead_values[dst.gid] = lw.astype(tv, rb_dtype(dst.dtype))
@@ -550,12 +542,14 @@ class deferred_op:
                 dead_values[dst.gid] = tv
         return ("ok", lw.finish(), gslots, aslots)
 
-    def _finish(self, live_gids):
-        for g in self.delete_gids:
+    def _finish(self, live):
+        """Free the blocks of the arrays that died while the op was pending; every other array the flush kept in memory
+        now has its blocks, at a fixed partition."""
+        for g in self.dead:
             RT.destroy_array(g)
-        for k in live_gids.keys():
-            if k not in self.delete_gids and bdarray.valid_gid(k):
-                bd = bdarray.get_by_gid(k)
+        for g in live:
+            if g not in self.dead:
+                bd = self.arrays[g].bd
                 bd.remote_constructed = True
                 bd.flex_dist = False
 
@@ -970,15 +964,13 @@ class ndarray:
             base, distribution, local_border, dtype = o.base if o.base is not None else o, o.distribution, o.local_border, o.dtype
             flex_dist, readonly, maskarray, shape = o.bdarray.flex_dist, o.readonly, o.maskarray, o.shape
         self.base = base
-        gid = None
-        if base is not None:
-            gid = base.gid
-            if base.readonly:
-                readonly = True
+        if base is not None and base.readonly:
+            readonly = True
         shape = shapeToInt(shape)
-        self.bdarray = bdarray.assign_bdarray(self, shape, gid, distribution, local_border, flex_dist, dtype, **kwargs)
+        self.bdarray = bdarray.assign_bdarray(self, shape, base.bdarray if base is not None else None, distribution, local_border,
+                                              flex_dist, dtype, **kwargs)
         self.shape = shape
-        self.distribution = distribution if (distribution is not None and gid is not None) else self.bdarray.distribution
+        self.distribution = distribution if (distribution is not None and base is not None) else self.bdarray.distribution
         self.local_border = local_border
         self.readonly = readonly
         self.maskarray = maskarray
@@ -1085,7 +1077,7 @@ class ndarray:
                 builtins.any(b != 1 and a != b for a, b in zip(shape[new_dims:], self.shape)):
             raise ValueError("Non-broadcastable.")
         bd = [i < new_dims or (shape[i] != 1 and self.shape[i - new_dims] == 1) for i in range(len(shape))]
-        if self.bdarray.flex_dist or not self.bdarray.remote_constructed:
+        if not self.bdarray.remote_constructed:
             DAG.instantiate(self)
         return ndarray(shape, base=self, distribution=shardview.broadcast(self.distribution, bd, shape),
                        local_border=0, readonly=True)
@@ -1230,7 +1222,7 @@ class ndarray:
             cindex = canonical_index(index, self.shape)
             DAG.instantiate(self)
             return getitem_global(self, tuple(s.start for s in cindex))
-        if self.bdarray.flex_dist or not self.bdarray.remote_constructed:
+        if not self.bdarray.remote_constructed:
             DAG.instantiate(self)
         # the partition of a slice view is a pure function of (this view's distribution, the index): computed once per
         # array and index - an iterative program takes the same slices every step (ramba/ramba.py:6548-6579 recomputes)
@@ -1298,7 +1290,7 @@ class ndarray:
             DAG.assign(view, value)
 
     def remapped_axis(self, newmap):
-        if self.bdarray.flex_dist or not self.bdarray.remote_constructed:
+        if not self.bdarray.remote_constructed:
             DAG.instantiate(self)
         newshape, newdist = shardview.remap_axis(self.shape, self.distribution, newmap)
         return ndarray(newshape, base=self, distribution=newdist, local_border=0, readonly=self.readonly)
@@ -1309,7 +1301,7 @@ class ndarray:
         axes = sorted(a % k for a in axes)
         if len(set(axes)) != len(axes):
             raise ValueError("repeated axis")
-        if self.bdarray.flex_dist or not self.bdarray.remote_constructed:
+        if not self.bdarray.remote_constructed:
             DAG.instantiate(self)
         newshape, newdist = shardview.expand_unit_dims(self.shape, self.distribution, axes)
         return ndarray(newshape, base=self, distribution=newdist, local_border=0, readonly=True)
