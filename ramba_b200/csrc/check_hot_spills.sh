@@ -3,7 +3,7 @@
 # loop and the dispatch loop.  ptxas runs this kernel at the 128-register cap; small source changes decide whether
 # loop-carried state stays in registers.  usage: check_hot_spills.sh build/rb200_elementwise_nd1.o
 o=$1
-cuobjdump -sass -fun '_ZN5rb20021vm_elementwise_kernelILi8ELi1ELb0EEEvNS_7KParamsE' $o | grep -E "^\s+/\*[0-9a-f]{4,}\*/" | sed 's/\/\* 0x[0-9a-f]* \*\///' > /tmp/hs.sass
+cuobjdump -sass -fun '_ZN5rb20021vm_elementwise_kernelILi8ELi1ELb0ELb0EEEvNS_7KParamsE' $o | grep -E "^\s+/\*[0-9a-f]{4,}\*/" | sed 's/\/\* 0x[0-9a-f]* \*\///' > /tmp/hs.sass
 total=$(wc -l < /tmp/hs.sass)
 h=$(grep -n "LDCU\?\.U16" /tmp/hs.sass | head -1 | cut -d: -f1)  # the load of the handler id opens the dispatch loop
 echo "total instrs $total; LDL/STL total $(grep -c 'LDL\|STL' /tmp/hs.sass); handler-load line $h"

@@ -151,13 +151,13 @@ static void assign_handlers(KParams& P, const rb200_fused_op* op, int set) {
 // ---- debugging aids (A/B measurements, bisecting a parity failure), read once: each takes a kernel family, the TMA
 // loader or the row tiling out of the selection, in the launch and in rb200_describe_plan alike
 struct KillSwitches {
-  bool no_tile, no_stream, no_mapred, no_terms, no_tma, no_row_mode, no_rng;
+  bool no_tile, no_stream, no_mapred, no_terms, no_tma, no_row_mode, no_rng, no_lean;
 };
 static const KillSwitches& kill_switches() {
   static const KillSwitches k = {getenv("RB200_NO_TILE_KERNEL") != nullptr,   getenv("RB200_NO_STREAM_KERNEL") != nullptr,
                                  getenv("RB200_NO_MAPRED_KERNEL") != nullptr, getenv("RB200_NO_TERMS_KERNEL") != nullptr,
                                  getenv("RB200_NO_TMA") != nullptr,           getenv("RB200_NO_ROW_MODE") != nullptr,
-                                 getenv("RB200_NO_RNG") != nullptr};
+                                 getenv("RB200_NO_RNG") != nullptr,           getenv("RB200_NO_LEAN_INTERP") != nullptr};
   return k;
 }
 
@@ -249,6 +249,7 @@ struct Plan {
   StreamPlan stream;  // FORM_STREAM
   RngPlan rng;        // FORM_RNG
   KParams k;          // the general interpreter forms
+  bool lean;          // FORM_ELEMENTWISE, 1-D: the lean instantiation (handler ids are lean ids)
   long long blocks;   // the general interpreter forms: grid and dynamic shared memory
   size_t smem;
   // axis reductions: the kernel writes splits [0, n_written) of n_split; launch() fills the rest with the identity
@@ -356,11 +357,31 @@ static bool plan_axis_as_1d(const rb200_fused_op* op, int sms, const bool* view_
   return true;
 }
 
+// The lean 1-D kernel (rb200_elementwise_lean.cu) runs a 1-D op list, already staged and given its set-1 handlers, when
+// every instruction has a handler of the lean set, nothing is reduced, every store is unmasked and goes to a contiguous
+// view of the result's own dtype, and the staged views move by bulk copies: what the lean kernel leaves out (the generic
+// path, reductions, converting / masked / strided stores, the per-thread staging pipeline) is then never needed.
+static bool lean_eligible(const KParams& P, const rb200_fused_op* op) {
+  if (P.ndim != 1 || op->n_reds != 0 || (P.n_pf > 0 && !P.bulk)) return false;
+  for (int i = 0; i < P.n_insns; ++i) {
+    const rb200_insn& I = P.insns[i];
+    const int h = P.handler[i];
+    if (h == H_GENERIC || kLeanOf1[h] == 0) return false;
+    if (I.st_view != RB200_NOSTORE && I.mask_reg != RB200_NOSTORE) return false;
+    const int own = I.ctype == RB200_T_F64 ? RB200_F64 : RB200_F32;  // the lean set is float64 / float32 only
+    const int stored[2] = {I.st_view, (I.op == RB200_OP_SINCOS && I.c_kind == RB200_K_VIEW) ? (int)I.c_idx : RB200_NOSTORE};
+    for (const int v : stored)
+      if (v != RB200_NOSTORE && (P.views[v].stride[0] != 1 || P.views[v].dtype != own)) return false;
+  }
+  return true;
+}
+
 // The kernel choice for a valid, non-empty op list on a device with `sms` multiprocessors.  The only decisions left to
 // the launch are the driver's: encoding a TMA tensor map (the cooperative loader when that fails).
 static void make_plan(const rb200_fused_op* op, int sms, Plan& pl) {
   const KillSwitches& ks = kill_switches();
   pl.form = FORM_NONE;
+  pl.lean = false;
   pl.n_split = pl.n_written = 0;
   // ---- a plain random draw (rb200_rng.cu): only op lists with a PHILOX instruction qualify
   if (!ks.no_rng && plan_rng(op, sms, pl.rng)) {
@@ -513,8 +534,13 @@ static void make_plan(const rb200_fused_op* op, int sms, Plan& pl) {
     }
     ocls_bytes = (size_t)P.n_ocls * V * kThreads * 8;
   }
-  const size_t smem = reg_bytes + pf_bytes + ocls_bytes;
   assign_handlers(P, op, op->ndim == 1 ? 1 : 2);
+  if (!ks.no_lean && lean_eligible(P, op)) {
+    pl.lean = true;
+    for (int i = 0; i < P.n_insns; ++i) P.handler[i] = kLeanOf1[P.handler[i]];
+  }
+  // (the lean kernel's stores never go through the scratch column behind the register file)
+  const size_t smem = (pl.lean ? reg_bytes - (size_t)V * kThreads * 8 : reg_bytes) + pf_bytes + ocls_bytes;
   if (op->n_reds > 0) {
     P.red_counter = (unsigned int*)op->red_scratch;
     P.red_partials = (u64*)((char*)op->red_scratch + 256);
@@ -560,8 +586,8 @@ static std::string launch_failure(const Plan& pl) {
     case FORM_AXIS_AS_1D: return "vm_elementwise_kernel (axis-as-1-D) launch";
     case FORM_AXIS_REDUCE: return "vm_axis_reduce_kernel launch";
     default:
-      snprintf(buf, sizeof(buf), "vm_elementwise_kernel launch (ndim=%d blocks=%lld smem=%zu n_regs=%d n_pf=%d n_insns=%d)", P.ndim, pl.blocks, pl.smem,
-               P.n_regs, P.n_pf, P.n_insns);
+      snprintf(buf, sizeof(buf), "vm_elementwise_kernel%s launch (ndim=%d blocks=%lld smem=%zu n_regs=%d n_pf=%d n_insns=%d)", pl.lean ? " (lean)" : "", P.ndim,
+               pl.blocks, pl.smem, P.n_regs, P.n_pf, P.n_insns);
   }
   return buf;
 }
@@ -581,7 +607,7 @@ static int launch(Plan& pl, cudaStream_t stream) {
     case FORM_AXIS_REDUCE: e = launch_vm_axis_reduce(P, blocks, pl.smem, stream); break;
     case FORM_ELEMENTWISE:
       switch (P.ndim) {
-        case 1: e = launch_vm_elementwise_nd1(P, blocks, pl.smem, stream); break;
+        case 1: e = pl.lean ? launch_vm_elementwise_lean(P, blocks, pl.smem, stream) : launch_vm_elementwise_nd1(P, blocks, pl.smem, stream); break;
         case 2: e = launch_vm_elementwise_nd2(P, blocks, pl.smem, stream); break;
         case 3: e = launch_vm_elementwise_nd3(P, blocks, pl.smem, stream); break;
         default: e = launch_vm_elementwise_nd5(P, blocks, pl.smem, stream); break;
@@ -609,8 +635,8 @@ static std::string describe(const rb200_fused_op* op, const Plan& pl) {
   const char* form = pl.form == FORM_ELEMENTWISE ? "elementwise" : pl.form == FORM_AXIS_AS_1D ? "axis_as_1d" : "axis_reduce";
   const char* tiling = pl.form != FORM_ELEMENTWISE || op->ndim == 1 ? "" : pl.k.row_chunks > 0 ? " tiling=row" : " tiling=flat";
   char buf[200];
-  snprintf(buf, sizeof(buf), "kernel=general_interpreter form=%s ndim=%d insns=%d views=%d%s ctas=%lld smem=%zu", form, op->ndim, op->n_insns, op->n_views,
-           tiling, pl.blocks, pl.smem);
+  snprintf(buf, sizeof(buf), "kernel=general_interpreter form=%s ndim=%d insns=%d views=%d%s ctas=%lld smem=%zu%s", form, op->ndim, op->n_insns,
+           op->n_views, tiling, pl.blocks, pl.smem, pl.lean ? " variant=lean" : "");
   return buf;
 }
 

@@ -13,23 +13,29 @@ namespace rb200 {
 // chunk: every thread keeps V column accumulators in registers across all its rows, views that are
 // broadcast over the rows are "periodic" (pf_slot == -2), and the per-CTA accumulators are written as
 // partials[(split)*C + column] with split = blockIdx / (C/TILE).
-template <int V, int ND, bool AX1D = false>
+// LEAN (ND == 1, rb200_elementwise_lean.cu): op lists of plain float arithmetic and sin / cos whose every instruction
+// has a handler of the lean set (rb200_handlers_lean.inc), with no reductions, unmasked stores to contiguous views of
+// the result's own dtype and every read view staged by bulk copies (the host checks all of it: lean_eligible in
+// rb200_api.cu).  The handler bodies are the full kernel's; without the generic path, the reductions and the
+// converting / masked stores, ptxas keeps the whole loop in registers.
+template <int V, int ND, bool AX1D = false, bool LEAN = false>
 #ifndef RB200_MIN_BLOCKS
 #define RB200_MIN_BLOCKS 2
 #endif
 __global__ void __launch_bounds__(kThreads, (ND == 1 && V <= 4) ? 3 : RB200_MIN_BLOCKS) vm_elementwise_kernel(const __grid_constant__ KParams P) {
+  static_assert(!LEAN || (ND == 1 && !AX1D), "the lean kernel is the plain 1-D one");
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ __align__(8) u64 mbar_store[4];
   constexpr int TILE = kThreads * V;
   constexpr unsigned SLOT = (unsigned)(TILE * 8);  // bytes reserved per staged view per stage
-  Ctx<V, ND> cx(P);
+  Ctx<V, ND, LEAN> cx(P);
   const unsigned smem_s = (unsigned)__cvta_generic_to_shared(smem);
   cx.tid = threadIdx.x;
   const int n_pf = (ND == 1) ? P.n_pf : 0;
   // layout: [prefetch stages 0..S-1][register file]  (stages first: 128-byte aligned)
   const unsigned pf_base = smem_s;
   const unsigned pf_stage_bytes = (unsigned)n_pf * SLOT;
-  const bool bulk = (ND == 1) && n_pf > 0 && P.bulk;
+  const bool bulk = (ND == 1) && n_pf > 0 && (LEAN || P.bulk);
   constexpr unsigned S = 2u;  // ring depth
   cx.regfile_s = smem_s + (n_pf > 0 ? S : 0u) * pf_stage_bytes + threadIdx.x * 8u;
   cx.ocls_s = cx.regfile_s + (unsigned)((P.n_regs + 1) * V * kThreads * 8);  // behind the register file and its scratch column  // offset-class table follows the register file
@@ -47,10 +53,12 @@ __global__ void __launch_bounds__(kThreads, (ND == 1 && V <= 4) ? 3 : RB200_MIN_
   constexpr int NS = 1;
   __shared__ u64 racc_extra[RB200_MAX_REDS - 1][kThreads];
   u64 racc[NS][AX1D ? V : 1];
+  if constexpr (!LEAN) {
 #pragma unroll
-  for (int k = 0; k < (AX1D ? V : 1); ++k) racc[0][k] = red_identity_bits(0 < P.n_reds ? P.reds[0].op : 0, 0 < P.n_reds ? P.reds[0].ctype : 0);
-  cx.racc_s = (unsigned)__cvta_generic_to_shared(&racc_extra[0][threadIdx.x]);
-  for (int s = 1; s < P.n_reds; ++s) racc_extra[s - 1][threadIdx.x] = red_identity_bits(P.reds[s].op, P.reds[s].ctype);
+    for (int k = 0; k < (AX1D ? V : 1); ++k) racc[0][k] = red_identity_bits(0 < P.n_reds ? P.reds[0].op : 0, 0 < P.n_reds ? P.reds[0].ctype : 0);
+    cx.racc_s = (unsigned)__cvta_generic_to_shared(&racc_extra[0][threadIdx.x]);
+    for (int s = 1; s < P.n_reds; ++s) racc_extra[s - 1][threadIdx.x] = red_identity_bits(P.reds[s].op, P.reds[s].ctype);
+  }
   if constexpr (AX1D) {
     cx.pe0 = (long long)(blockIdx.x % (unsigned)P.n_split_chunks) * TILE + threadIdx.x;
     cx.e0 = cx.pe0;
@@ -235,8 +243,9 @@ __global__ void __launch_bounds__(kThreads, (ND == 1 && V <= 4) ? 3 : RB200_MIN_
     }
     cx.valid = valid;
     cx.fill_offset_classes();
-    run_program<V, AX1D, NS>(cx, racc);
+    run_program<V, AX1D, NS, LEAN>(cx, racc);
   }
+  if constexpr (LEAN) return;
   if (n_pf > 0 && !bulk) cp_async_wait<0>();
 
   if constexpr (AX1D) {
@@ -312,12 +321,13 @@ __global__ void __launch_bounds__(kThreads, (ND == 1 && V <= 4) ? 3 : RB200_MIN_
   }
 }
 
-template <int V, int ND, bool AX1D = false> cudaError_t launch_vm_elementwise_nd(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream) {
+template <int V, int ND, bool AX1D = false, bool LEAN = false>
+cudaError_t launch_vm_elementwise_nd(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream) {
   if (smem + 2048 > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(vm_elementwise_kernel<V, ND, AX1D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(vm_elementwise_kernel<V, ND, AX1D, LEAN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
   }
-  vm_elementwise_kernel<V, ND, AX1D><<<blocks, kThreads, smem, stream>>>(P);
+  vm_elementwise_kernel<V, ND, AX1D, LEAN><<<blocks, kThreads, smem, stream>>>(P);
   return cudaGetLastError();
 }
 

@@ -126,7 +126,7 @@ __device__ __noinline__ void store_slow_nd(char* base, int dtype, unsigned mask,
 // ---------------------------------------------------------------------------------------------
 // per-thread interpreter state.  ND = number of iteration dims this instantiation handles
 // (ND == 1: collapsed 1-D op, the hot path; element k of the thread is e0 + k*256).
-template <int V, int ND> struct Ctx {
+template <int V, int ND, bool LEAN = false> struct Ctx {
   static constexpr int kND = ND;
   const KParams& P;      // the __grid_constant__ kernel parameter: constant-bank (LDC) accesses
   unsigned regfile_s;    // shared-window byte address of this thread's column of the register file
@@ -287,7 +287,18 @@ template <int V, int ND> struct Ctx {
   // store V results (values r, raw bits b) to view `vi`, optionally masked by register `mreg`:
   // full contiguous tiles of the view's own dtype inline, everything else out of line
   template <class R> __device__ __forceinline__ void store_res(int vi, int mreg, const R (&r)[V], const u64 (&b)[V]) {
-    if constexpr (ND == 1 && (V == 4 || V == 8)) {
+    if constexpr (LEAN) {
+      // the lean kernel stores only unmasked, to contiguous views of the result's own dtype (host-checked)
+      R* p = reinterpret_cast<R*>(P.views[vi].base) + e0;
+      if (valid == ((1u << V) - 1u)) {
+#pragma unroll
+        for (int k = 0; k < V; ++k) stg<R>(p + k * kThreads, r[k]);
+      } else {  // the ragged last tile
+#pragma unroll
+        for (int k = 0; k < V; ++k)
+          if ((valid >> k) & 1u) stg<R>(p + k * kThreads, r[k]);
+      }
+    } else if constexpr (ND == 1 && (V == 4 || V == 8)) {
       const KView& vw = P.views[vi];
       constexpr int own1 = std::is_same<R, double>::value ? RB200_F64 : std::is_same<R, float>::value ? RB200_F32 : RB200_I64;
       const long long st = vw.stride[0];
@@ -1042,7 +1053,7 @@ template <int V, bool AX, int NS, class C> __device__ __noinline__ void generic_
 // one interpreter pass over the op list for the thread's V elements.
 // racc: reduction accumulators (raw bits), [slot][0] (global mode, AX=false) or [slot][k] (axis mode)
 // NS = number of reduction slots carried in registers
-template <int V, bool AX, int NS, class C> __device__ __forceinline__ void run_program(C& cx, u64 (&racc)[NS][AX ? V : 1]) {
+template <int V, bool AX, int NS, bool LEAN = false, class C> __device__ __forceinline__ void run_program(C& cx, u64 (&racc)[NS][AX ? V : 1]) {
   const KParams& P = cx.P;
   const int n = P.n_insns;
   const unsigned valid_tile = cx.valid;
@@ -1060,27 +1071,31 @@ template <int V, bool AX, int NS, class C> __device__ __forceinline__ void run_p
     }
 #ifndef RB200_NO_FAST_HANDLERS
     const int h = P.handler[pc];
-    if (h != H_GENERIC) {
+    if constexpr (LEAN) {  // lean handler ids (kLeanOf1); the host admits no instruction outside the lean set
+#include "rb200_handlers_lean.inc"
+    } else {
+      if (h != H_GENERIC) {
 #if RB200_HANDLER_SET == 2
 #include "rb200_handlers_set2.inc"
 #else
 #include "rb200_handlers_set1.inc"
 #endif
-      continue;
-    }
-    {
-      u64 acc_tmp[V], racc_tmp[NS * (AX ? V : 1)];
+        continue;
+      }
+      {
+        u64 acc_tmp[V], racc_tmp[NS * (AX ? V : 1)];
 #pragma unroll
-      for (int s = 0; s < NS; ++s)
+        for (int s = 0; s < NS; ++s)
 #pragma unroll
-        for (int k = 0; k < (AX ? V : 1); ++k) racc_tmp[s * (AX ? V : 1) + k] = racc[s][k];
-      generic_step<V, AX, NS, C>(cx, pc, acc_tmp, racc_tmp);
+          for (int k = 0; k < (AX ? V : 1); ++k) racc_tmp[s * (AX ? V : 1) + k] = racc[s][k];
+        generic_step<V, AX, NS, C>(cx, pc, acc_tmp, racc_tmp);
 #pragma unroll
-      for (int k = 0; k < V; ++k) cx.acc[k] = acc_tmp[k];
+        for (int k = 0; k < V; ++k) cx.acc[k] = acc_tmp[k];
 #pragma unroll
-      for (int s = 0; s < NS; ++s)
+        for (int s = 0; s < NS; ++s)
 #pragma unroll
-        for (int k = 0; k < (AX ? V : 1); ++k) racc[s][k] = racc_tmp[s * (AX ? V : 1) + k];
+          for (int k = 0; k < (AX ? V : 1); ++k) racc[s][k] = racc_tmp[s * (AX ? V : 1) + k];
+      }
     }
 #else
     generic_body<V, AX, NS>(cx, I, racc);

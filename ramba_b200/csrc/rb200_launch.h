@@ -9,6 +9,7 @@ cudaError_t launch_vm_elementwise_nd1(const KParams& P, unsigned blocks, size_t 
 cudaError_t launch_vm_elementwise_nd2(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream);
 cudaError_t launch_vm_elementwise_nd3(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream);
 cudaError_t launch_vm_elementwise_nd5(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream);
+cudaError_t launch_vm_elementwise_lean(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream);
 cudaError_t launch_vm_elementwise_ax1d(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream);
 cudaError_t launch_vm_axis_reduce(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream);
 long long scan_scratch_bytes(long long n_outer, long long len, long long n_inner);
