@@ -15,8 +15,8 @@ namespace rb200 {
 // partials[(split)*C + column] with split = blockIdx / (C/TILE).
 // LEAN (ND == 1, rb200_elementwise_lean.cu): op lists of plain float arithmetic and sin / cos whose every instruction
 // has a handler of the lean set (rb200_handlers_lean.inc), with no reductions, unmasked stores to contiguous views of
-// the result's own dtype and every read view staged by bulk copies (the host checks all of it: lean_eligible in
-// rb200_api.cu).  The handler bodies are the full kernel's; without the generic path, the reductions and the
+// the result's own dtype and every read view staged by bulk copies (the host checks all of it: lean_interp_eligible in
+// rb200_interp_plan.cu).  The handler bodies are the full kernel's; without the generic path, the reductions and the
 // converting / masked stores, ptxas keeps the whole loop in registers.
 template <int V, int ND, bool AX1D = false, bool LEAN = false>
 #ifndef RB200_MIN_BLOCKS

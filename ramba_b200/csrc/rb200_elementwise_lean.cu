@@ -1,5 +1,5 @@
 // rb200_elementwise_lean.cu — the lean instantiation of the 1-D elementwise kernel (lean handler set only; see
-// vm_elementwise_kernel in rb200_elementwise.cuh and lean_eligible in rb200_api.cu).
+// vm_elementwise_kernel in rb200_elementwise.cuh and lean_interp_eligible in rb200_interp_plan.cu).
 #include "rb200_elementwise.cuh"
 namespace rb200 {
 cudaError_t launch_vm_elementwise_lean(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream) {

@@ -1,4 +1,6 @@
 #pragma once
+#include <string>
+
 #include "rb200_vm.cuh"
 
 namespace rb200 {
@@ -12,6 +14,23 @@ cudaError_t launch_vm_elementwise_nd5(const KParams& P, unsigned blocks, size_t 
 cudaError_t launch_vm_elementwise_lean(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream);
 cudaError_t launch_vm_elementwise_ax1d(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream);
 cudaError_t launch_vm_axis_reduce(const KParams& P, unsigned blocks, size_t smem, cudaStream_t stream);
+
+// the general interpreter's plan (rb200_interp_plan.cu): an elementwise op list (with global reductions) or an axis
+// reduction; for the axis forms the kernel writes splits [0, n_written) of the requested ones
+enum InterpForm { INTERP_ELEMENTWISE, INTERP_AXIS_AS_1D, INTERP_AXIS_REDUCE };
+struct InterpPlan {
+  InterpForm form;
+  KParams k;
+  bool lean;  // INTERP_ELEMENTWISE, 1-D: the lean instantiation (handler ids are lean ids)
+  long long blocks;
+  size_t smem;
+  int n_written;
+};
+// any valid, non-empty op list.  row_mode / lean: the N-d row tiling and the lean 1-D kernel may be chosen
+void plan_interp(const rb200_fused_op* op, int sms, bool row_mode, bool lean, InterpPlan& I);
+// one line for rb200_describe_plan
+std::string describe_interp(const rb200_fused_op* op, const InterpPlan& I);
+
 long long scan_scratch_bytes(long long n_outer, long long len, long long n_inner);
 cudaError_t launch_scan(const void* src, void* dst, int dtype, long long n_outer, long long len, long long n_inner, int op, const void* carry, void* totals,
                         void* scratch, int sms, cudaStream_t stream, bool* supported);

@@ -3,7 +3,7 @@
 // What it stands for in the reference: the generated loop `for index in numba.pndindex(itershape): ...` over a
 // contiguous 1-D (collapsed) iteration space (ramba/ramba.py:8246-8255), with the pre/postcode of a global reduction
 // (`red[0] = red[0] + acc`, ramba/ramba.py:5798-5807), and the axis-reduction loop nest over a [rows][columns] box
-// (ramba/ramba.py:8231-8244) - for op lists made of plain float arithmetic (rb200_lean_plan.h).  Affine maps feeding
+// (ramba/ramba.py:8231-8244) - for op lists made of plain float arithmetic (rb200_plan.h).  Affine maps feeding
 // a sum (`(X*2.0 + 1.0).sum()`), broadcast-add + column sums (`(M + v).sum(axis=0)`), float32 streams in general:
 // at 4 bytes per element the general interpreter is bound by its own dispatch cost, this kernel by HBM.
 //
@@ -25,7 +25,7 @@
 
 #include "rb200_launch.h"
 #include "rb200_lean.cuh"
-#include "rb200_lean_plan.h"
+#include "rb200_plan.h"
 #include "rb200_terms.h"
 #include "rb200_mapred.h"
 #include "rb200_stream.h"
@@ -702,18 +702,11 @@ __global__ void __launch_bounds__(kThreads, TV == 8 ? RB200_STREAM_MINB8 : 2) st
 // =============================================================================================
 // host side
 
-static bool stream_translate(const rb200_fused_op* op, StreamParams& P, bool column_mode, long long row_len) {
+// the view tables; view_kind / view_arg / store_arg: how lean_translate addresses each view
+static void stream_views(const rb200_fused_op* op, StreamParams& P, bool column_mode, long long row_len, int* view_kind, int* view_arg, int* store_arg) {
   // staged: read views that are contiguous along the iteration (and, in column mode, over the rows) with 16-byte
   // aligned tiles; everything else direct
-  bool rd[RB200_MAX_VIEWS] = {false};
-  for (int i = 0; i < op->n_insns; ++i) {
-    const rb200_insn& I = op->insns[i];
-    const int lop = lean_opcode(op, I);
-    if (I.a_kind == RB200_K_VIEW) rd[I.a_idx] = true;
-    if (I.b_kind == RB200_K_VIEW && lop != LO_RED && lop != LO_SQUARE) rd[I.b_idx] = true;
-    if (I.c_kind == RB200_K_VIEW) rd[I.c_idx] = true;
-  }
-  int view_kind[RB200_MAX_VIEWS], view_arg[RB200_MAX_VIEWS], store_arg[RB200_MAX_VIEWS];
+  const ViewUse use = view_use(op);
   unsigned off = 0;
   for (int v = 0; v < op->n_views; ++v) {
     const rb200_view& vw = op->views[v];
@@ -728,7 +721,7 @@ static bool stream_translate(const rb200_fused_op* op, StreamParams& P, bool col
     view_arg[v] = store_arg[v] = P.n_direct;
     const bool contiguous = d.s2 == 1 && (!column_mode || d.s1 == row_len);
     const bool aligned = (((uintptr_t)vw.base) & 15u) == 0 && (!column_mode || (row_len * es) % 16 == 0);
-    if (rd[v] && contiguous && aligned && P.n_staged < kStreamMaxStaged) {
+    if (use.read[v] && contiguous && aligned && P.n_staged < kStreamMaxStaged) {
       StreamStaged& s = P.staged[P.n_staged];
       s.base = (const char*)vw.base;
       s.es = es;
@@ -744,43 +737,8 @@ static bool stream_translate(const rb200_fused_op* op, StreamParams& P, bool col
   P.stage_bytes = off;
   P.n_insns = op->n_insns;
   P.n_regs = op->n_regs;
-  lean_translate(op, view_kind, view_arg, store_arg, P.insns);
   for (int i = 0; i < op->n_scalars; ++i) P.scal[i] = op->scalars[i];
-  return true;
 }
-
-// lean kernel, column mode: row-broadcast operands fetched in ONE class move into the register file
-static void stream_hoist_lean(StreamParams& P) {
-    for (int dv = 0; dv < P.n_direct && P.n_hoist < kStreamMaxStaged; ++dv) {
-      if (P.direct[dv].s1 != 0 || P.direct[dv].s2 != 1) continue;
-      int cls = -1;
-      bool same = true, used = false;
-      for (int i = 0; i < P.n_insns; ++i) {
-        const LInsn& L = P.insns[i];
-        const int lop = L.handler >> 2;
-        int fcls = (L.handler >> 1) & 1;  // 1: f32
-        if (lop == LO_CVT) fcls = 1 - fcls;  // CVT fetches its operand in the OTHER class
-        const bool uses = (L.a_kind == L_DIRECT && L.a_arg == dv) || (L.b_kind == L_DIRECT && L.b_arg == dv) || (L.c_kind == L_DIRECT && L.c_arg == dv);
-        if (!uses) continue;
-        used = true;
-        if (cls < 0) cls = fcls;
-        else if (cls != fcls) same = false;
-      }
-      if (!used || !same) continue;
-      const int reg = P.n_regs + P.n_hoist;
-      if (reg >= 255) break;
-      P.hoist[P.n_hoist].direct = dv;
-      P.hoist[P.n_hoist].reg = reg;
-      P.hoist[P.n_hoist].is_f32_class = cls;
-      ++P.n_hoist;
-      for (int i = 0; i < P.n_insns; ++i) {
-        LInsn& L = P.insns[i];
-        if (L.a_kind == L_DIRECT && L.a_arg == dv) { L.a_kind = L_REG; L.a_arg = (unsigned char)reg; }
-        if (L.b_kind == L_DIRECT && L.b_arg == dv) { L.b_kind = L_REG; L.b_arg = (unsigned char)reg; }
-        if (L.c_kind == L_DIRECT && L.c_arg == dv) { L.c_kind = L_REG; L.c_arg = (unsigned char)reg; }
-      }
-    }
-  }
 
 // byte offsets of the staged views inside a stage for tiles of tv * 256 elements
 static void stream_layout(StreamParams& P) {
@@ -808,13 +766,13 @@ static size_t stream_smem(StreamParams& P) {
   return (size_t)depth * P.stage_bytes + regs + (size_t)(depth > 0 ? depth : 1) * 8 + 16;
 }
 
-bool plan_stream(const rb200_fused_op* op, int sms, int max_red_blocks, int n_split, bool use_terms, bool use_mapred, StreamPlan& T) {
+bool plan_stream(const rb200_fused_op* op, int sms, int n_split, bool use_terms, bool use_mapred, StreamPlan& T) {
   StreamParams& P = T.P;
   memset(&T, 0, sizeof(T));
   const bool column = op->n_axis_red_dims != 0;
   if (!column) {
     if (op->ndim != 1) return false;
-    if (!lean_eligible(op, true)) return false;
+    if (!lean_vocabulary_only(op, true)) return false;
     for (int s = 0; s < op->n_reds; ++s) {
       if (op->reds[s].ctype != RB200_T_F64) return false;
       if (op->reds[s].out_dtype != RB200_F64 && op->reds[s].out_dtype != RB200_F32) return false;
@@ -823,7 +781,7 @@ bool plan_stream(const rb200_fused_op* op, int sms, int max_red_blocks, int n_sp
     P.total = op->itershape[0];
   } else {
     if (op->ndim != 2 || op->n_axis_red_dims != 1 || op->n_reds != 1) return false;
-    if (!lean_eligible(op, true)) return false;
+    if (!lean_vocabulary_only(op, true)) return false;
     if (op->reds[0].ctype != RB200_T_F64) return false;
     const long long R = op->itershape[0], C = op->itershape[1];
     if (C % (LV * kThreads) != 0 || R < 2) return false;
@@ -839,7 +797,9 @@ bool plan_stream(const rb200_fused_op* op, int sms, int max_red_blocks, int n_sp
     P.total = R * C;
   }
   P.tv = LV;
-  stream_translate(op, P, column, P.C);
+  int view_kind[RB200_MAX_VIEWS], view_arg[RB200_MAX_VIEWS], store_arg[RB200_MAX_VIEWS];
+  stream_views(op, P, column, P.C, view_kind, view_arg, store_arg);
+  lean_translate(op, op->insns, view_kind, view_arg, store_arg, P.insns);
   // ---- the term form first
   TermBuild tb;
   tb.n_regs = P.n_regs;
@@ -869,15 +829,11 @@ bool plan_stream(const rb200_fused_op* op, int sms, int max_red_blocks, int n_sp
       bool ok = true;
       if (!column) {
         M.total = P.total;
-        M.red.op = op->reds[0].op;
-        M.red.ctype = op->reds[0].ctype;
-        M.red.out = op->reds[0].out;
-        M.red.out_dtype = op->reds[0].out_dtype;
-        M.red_counter = (unsigned int*)op->red_scratch;
-        M.red_partials = (u64*)((char*)op->red_scratch + 256);
+        bind_reds(op, &M.red);
+        bind_red_scratch(op, &M.red_counter, &M.red_partials);
         long long blocks = (P.total / (vec * 4) + kThreads - 1) / kThreads;
         long long cap = (long long)sms * 8;
-        if (cap > max_red_blocks) cap = max_red_blocks;
+        if (cap > kRedScratchPartials) cap = kRedScratchPartials;
         if (blocks > cap) blocks = cap;
         if (blocks < 1) blocks = 1;
         T.blocks = blocks;
@@ -888,10 +844,7 @@ bool plan_stream(const rb200_fused_op* op, int sms, int max_red_blocks, int n_sp
           M.R = P.R;
           M.C = P.C;
           M.n_chunks = (int)(P.C / chunk);
-          int eff = (int)(((long long)sms * 8) / M.n_chunks);
-          if (n_split > 0 && eff > n_split) eff = n_split;
-          if ((long long)eff > P.R) eff = (int)P.R;
-          if (eff < 1) eff = 1;
+          const int eff = row_split((long long)sms * 8, M.n_chunks, n_split, P.R);
           M.n_split = eff;
           M.rows_per_split = (P.R + eff - 1) / eff;
           M.red_partials = (u64*)op->red_scratch;
@@ -926,37 +879,35 @@ bool plan_stream(const rb200_fused_op* op, int sms, int max_red_blocks, int n_sp
     }
   } else {
     P.n_terms = 0;
-    if (column) stream_hoist_lean(P);
+    if (column) {
+      // the lean kernel: row-broadcast operands fetched in one class move into the register file, so the list is
+      // translated again from a hoisted copy (the term form above reads them from the direct views)
+      rb200_insn insns[RB200_MAX_INSNS];
+      memcpy(insns, op->insns, sizeof(rb200_insn) * op->n_insns);
+      int view[kStreamMaxStaged], reg[kStreamMaxStaged], cls[kStreamMaxStaged];
+      P.n_hoist = hoist_row_broadcast(op, insns, P.n_regs, 255, kStreamMaxStaged, view, reg, cls);
+      for (int j = 0; j < P.n_hoist; ++j) P.hoist[j] = {view[j], reg[j], cls[j] == RB200_T_F32};
+      lean_translate(op, insns, view_kind, view_arg, store_arg, P.insns);
+    }
   }
   T.smem = stream_smem(P);
   if (T.smem == 0) return false;
   const long long tile = (long long)P.tv * kThreads;
   P.n_reds = op->n_reds;
-  for (int s = 0; s < op->n_reds; ++s) {
-    P.reds[s].op = op->reds[s].op;
-    P.reds[s].ctype = op->reds[s].ctype;
-    P.reds[s].out = op->reds[s].out;
-    P.reds[s].out_dtype = op->reds[s].out_dtype;
-  }
+  bind_reds(op, P.reds);
   if (!column) {
     P.n_tiles = (P.total + tile - 1) / tile;
-    if (op->n_reds > 0) {
-      P.red_counter = (unsigned int*)op->red_scratch;
-      P.red_partials = (u64*)((char*)op->red_scratch + 256);
-    }
+    if (op->n_reds > 0) bind_red_scratch(op, &P.red_counter, &P.red_partials);
     long long blocks = P.n_tiles;
     long long cap = (long long)sms * ((P.n_terms > 0 && T.smem <= 72 * 1024) ? RB200_STREAM_MINB8 : 2);
-    if (op->n_reds > 0 && cap > max_red_blocks) cap = max_red_blocks;
+    if (op->n_reds > 0 && cap > kRedScratchPartials) cap = kRedScratchPartials;
     if (blocks > cap) blocks = cap;
     T.blocks = blocks;
   } else {
     P.n_chunks = (int)(P.C / tile);
     const int per_sm = (P.n_terms > 0 && T.smem <= 72 * 1024) ? RB200_STREAM_MINB8 : 2;
     if (P.n_chunks > sms * per_sm) return false;
-    int eff = (int)(((long long)sms * per_sm) / P.n_chunks);
-    if (n_split > 0 && eff > n_split) eff = n_split;
-    if ((long long)eff > P.R) eff = (int)P.R;
-    if (eff < 1) eff = 1;
+    const int eff = row_split((long long)sms * per_sm, P.n_chunks, n_split, P.R);
     P.n_split = eff;
     P.rows_per_split = (P.R + eff - 1) / eff;
     P.red_partials = (u64*)op->red_scratch;

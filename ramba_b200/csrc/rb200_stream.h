@@ -66,7 +66,7 @@ struct StreamPlan {
 // mode 0 (a contiguous 1-D space, optional global reductions) or mode 1 (one axis reduction over the rows of a [R][C]
 // box into n_split row slices; T.eff of them are written).  false: the op list is not of this form.  use_terms /
 // use_mapred: the term kernel and the map + reduce kernels may be chosen
-bool plan_stream(const rb200_fused_op* op, int sms, int max_red_blocks, int n_split, bool use_terms, bool use_mapred, StreamPlan& T);
+bool plan_stream(const rb200_fused_op* op, int sms, int n_split, bool use_terms, bool use_mapred, StreamPlan& T);
 // one line for rb200_describe_plan
 std::string describe_stream(const StreamPlan& T);
 cudaError_t launch_stream(const StreamPlan& T, cudaStream_t stream);

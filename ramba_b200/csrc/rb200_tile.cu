@@ -31,7 +31,7 @@
 
 #include "rb200_launch.h"
 #include "rb200_lean.cuh"
-#include "rb200_lean_plan.h"
+#include "rb200_plan.h"
 #include "rb200_terms.h"
 #include "rb200_tile.h"
 
@@ -561,7 +561,7 @@ static long long floor_div(long long a, long long b) {  // b > 0
 bool plan_stencil_tile(const rb200_fused_op* op, int sms, bool use_terms, bool use_tma, TilePlan& T) {
   if (op->ndim != 2 && op->ndim != 3) return false;
   if (op->n_reds != 0 || op->n_axis_red_dims != 0) return false;
-  if (!lean_eligible(op, false)) return false;
+  if (!lean_vocabulary_only(op, false)) return false;
   const int nd = op->ndim;
   TileParams& P = T.P;
   memset(&T, 0, sizeof(T));
@@ -570,19 +570,29 @@ bool plan_stencil_tile(const rb200_fused_op* op, int sms, bool use_terms, bool u
   P.X = op->itershape[nd - 1];
   if (P.X >= (1ll << 31) || P.Y >= (1ll << 31) || P.Z >= (1ll << 31)) return false;
 
-  // ---- which views are read / written
-  bool rd[RB200_MAX_VIEWS] = {false}, wr[RB200_MAX_VIEWS] = {false};
-  for (int i = 0; i < op->n_insns; ++i) {
-    const rb200_insn& I = op->insns[i];
-    const int lop = lean_opcode(op, I);
-    if (I.a_kind == RB200_K_VIEW) rd[I.a_idx] = true;
-    if (I.b_kind == RB200_K_VIEW && lop != LO_RED && lop != LO_SQUARE) rd[I.b_idx] = true;
-    if (I.c_kind == RB200_K_VIEW) rd[I.c_idx] = true;
-    if (I.st_view != RB200_NOSTORE) wr[I.st_view] = true;
-  }
+  const ViewUse use = view_use(op);
   auto S = [&](int v, int d) -> long long {  // stride of normalised dim d (0 = z, 1 = y, 2 = x)
     if (nd == 3) return op->views[v].stride[d];
     return d == 0 ? 0 : op->views[v].stride[d - 1];
+  };
+  // the shift of view v from the reference view r, when v is a member of r's group: read-only, r's dtype, strides and
+  // allocation, and a base offset that decomposes into a shift within +-3 planes, +-8 rows and +-8 columns
+  auto group_shift = [&](int v, int r, long long* dz, long long* dy, long long* dx) -> bool {
+    if (!use.read[v] || use.written[v] || op->views[v].dtype != op->views[r].dtype) return false;
+    if (S(v, 0) != S(r, 0) || S(v, 1) != S(r, 1) || S(v, 2) != 1) return false;
+    if (op->views[v].alloc_lo != op->views[r].alloc_lo) return false;
+    const int es = op->views[r].dtype == RB200_F64 ? 8 : 4;
+    const long long db = (const char*)op->views[v].base - (const char*)op->views[r].base;
+    if (db % es != 0) return false;
+    long long delta = db / es;
+    *dz = 0;
+    if (nd == 3 && S(r, 0) > 0) {
+      *dz = floor_div(delta + S(r, 0) / 2, S(r, 0));
+      delta -= *dz * S(r, 0);
+    }
+    *dy = floor_div(delta + S(r, 1) / 2, S(r, 1));
+    *dx = delta - *dy * S(r, 1);
+    return *dz >= -3 && *dz <= 3 && *dy >= -8 && *dy <= 8 && *dx >= -8 && *dx <= 8;
   };
 
   // ---- staged group: the largest family of read-only views with equal dtype and strides (unit x stride) whose base
@@ -591,26 +601,12 @@ bool plan_stencil_tile(const rb200_fused_op* op, int sms, bool use_terms, bool u
   int member[RB200_MAX_VIEWS];
   long long mdz[RB200_MAX_VIEWS], mdy[RB200_MAX_VIEWS], mdx[RB200_MAX_VIEWS];
   for (int r = 0; r < op->n_views; ++r) {
-    if (!rd[r] || wr[r] || S(r, 2) != 1 || S(r, 1) < 64 || (nd == 3 && S(r, 0) < S(r, 1))) continue;
+    if (!use.read[r] || use.written[r] || S(r, 2) != 1 || S(r, 1) < 64 || (nd == 3 && S(r, 0) < S(r, 1))) continue;
     if (!op->views[r].alloc_lo || !op->views[r].alloc_hi) continue;
-    const int es = op->views[r].dtype == RB200_F64 ? 8 : 4;
     int n = 0;
-    for (int v = 0; v < op->n_views; ++v) {
-      if (!rd[v] || wr[v] || op->views[v].dtype != op->views[r].dtype) continue;
-      if (S(v, 0) != S(r, 0) || S(v, 1) != S(r, 1) || S(v, 2) != 1) continue;
-      if (op->views[v].alloc_lo != op->views[r].alloc_lo) continue;
-      const long long db = (const char*)op->views[v].base - (const char*)op->views[r].base;
-      if (db % es != 0) continue;
-      long long delta = db / es, dz = 0;
-      if (nd == 3 && S(r, 0) > 0) {
-        dz = floor_div(delta + S(r, 0) / 2, S(r, 0));
-        delta -= dz * S(r, 0);
-      }
-      const long long dy = floor_div(delta + S(r, 1) / 2, S(r, 1));
-      const long long dx = delta - dy * S(r, 1);
-      if (dz < -3 || dz > 3 || dy < -8 || dy > 8 || dx < -8 || dx > 8) continue;
-      ++n;
-    }
+    long long dz, dy, dx;
+    for (int v = 0; v < op->n_views; ++v)
+      if (group_shift(v, r, &dz, &dy, &dx)) ++n;
     if (n > best_n) {
       best_n = n;
       best_ref = r;
@@ -629,19 +625,8 @@ bool plan_stencil_tile(const rb200_fused_op* op, int sms, bool use_terms, bool u
     long long lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0};
     int n = 0;
     for (int v = 0; v < op->n_views; ++v) {
-      if (!rd[v] || wr[v] || op->views[v].dtype != op->views[r].dtype) continue;
-      if (S(v, 0) != S(r, 0) || S(v, 1) != S(r, 1) || S(v, 2) != 1) continue;
-      if (op->views[v].alloc_lo != op->views[r].alloc_lo) continue;
-      const long long db = (const char*)op->views[v].base - (const char*)op->views[r].base;
-      if (db % es != 0) continue;
-      long long delta = db / es, dz = 0;
-      if (nd == 3 && S(r, 0) > 0) {
-        dz = floor_div(delta + S(r, 0) / 2, S(r, 0));
-        delta -= dz * S(r, 0);
-      }
-      const long long dy = floor_div(delta + S(r, 1) / 2, S(r, 1));
-      const long long dx = delta - dy * S(r, 1);
-      if (dz < -3 || dz > 3 || dy < -8 || dy > 8 || dx < -8 || dx > 8) continue;
+      long long dz, dy, dx;
+      if (!group_shift(v, r, &dz, &dy, &dx)) continue;
       member[n] = v;
       mdz[n] = dz; mdy[n] = dy; mdx[n] = dx;
       if (dz < lo[0]) lo[0] = dz;
@@ -698,7 +683,7 @@ bool plan_stencil_tile(const rb200_fused_op* op, int sms, bool use_terms, bool u
   }
   P.n_insns = op->n_insns;
   P.n_regs = op->n_regs;
-  lean_translate(op, view_kind, view_arg, store_arg, P.insns);
+  lean_translate(op, op->insns, view_kind, view_arg, store_arg, P.insns);
   P.tv = LV;
   TermBuild tb;
   tb.n_regs = P.n_regs;
