@@ -54,6 +54,49 @@ struct LDirect {  // a view addressed in global memory: element (z, y, x) at bas
   int pad;
 };
 
+// N elements of a direct view, element k at element offset off + k * step; elements outside `valid` read as 0
+template <class F, int N>
+__device__ __forceinline__ void ldirect_load(const LDirect& v, long long off, long long step, unsigned valid, F (&out)[N]) {
+  if (v.dtype == RB200_F32) {
+    const float* p = reinterpret_cast<const float*>(v.base) + off;
+#pragma unroll
+    for (int k = 0; k < N; ++k, p += step) out[k] = ((valid >> k) & 1u) ? (F)ldg<float>(p) : F(0);
+  } else {
+    const double* p = reinterpret_cast<const double*>(v.base) + off;
+#pragma unroll
+    for (int k = 0; k < N; ++k, p += step) out[k] = ((valid >> k) & 1u) ? (F)ldg<double>(p) : F(0);
+  }
+}
+
+// N values rounded to S, value k stored at p + k * step (step in units of *p: elements of S, or bytes for a char*);
+// only elements inside `valid` are written.  full: all N are, one unpredicated loop.
+template <class S, class F, int N, class Ptr>
+__device__ __forceinline__ void store_strided(Ptr p, long long step, bool full, unsigned valid, const F (&r)[N]) {
+  if (full) {
+#pragma unroll
+    for (int k = 0; k < N; ++k, p += step) stg<S>(reinterpret_cast<S*>(p), (S)r[k]);
+  } else {
+#pragma unroll
+    for (int k = 0; k < N; ++k, p += step)
+      if ((valid >> k) & 1u) stg<S>(reinterpret_cast<S*>(p), (S)r[k]);
+  }
+}
+
+// the addressing of ldirect_load for a store, rounded to the view's dtype
+template <class F, int N>
+__device__ __forceinline__ void ldirect_store(const LDirect& v, long long off, long long step, unsigned valid, const F (&r)[N]) {
+  if (v.dtype == RB200_F32) store_strided<float>(reinterpret_cast<float*>(v.base) + off, step, false, valid, r);
+  else store_strided<double>(reinterpret_cast<double*>(v.base) + off, step, false, valid, r);
+}
+
+// the same store by byte address and byte step, with the unpredicated loop when all N elements are valid (the term
+// kernels walk their output this way)
+template <class F, int N> __device__ __forceinline__ void store_bytes(char* p, long long step, int dtype, unsigned valid, const F (&r)[N]) {
+  constexpr unsigned all = N == 32 ? 0xffffffffu : (1u << N) - 1u;
+  if (dtype == RB200_F32) store_strided<float>(p, step, valid == all, valid, r);
+  else store_strided<double>(p, step, valid == all, valid, r);
+}
+
 // ---- register-level accumulator: low / high words kept apart so that float values cost one register
 template <class F> struct LAcc;
 template <> struct LAcc<double> {
@@ -76,6 +119,39 @@ template <> __device__ __forceinline__ void lean_sts<double>(unsigned addr, doub
 template <> __device__ __forceinline__ void lean_sts<float>(unsigned addr, float v) {
   asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(__float_as_uint(v)) : "memory");
 }
+
+// a scalar operand (raw bits of its class) as a value of class F
+template <class F> __device__ __forceinline__ F scal_as(u64 bits) {
+  return sizeof(F) == 8 ? (F)__longlong_as_double((long long)bits) : (F)__uint_as_float((unsigned)bits);
+}
+
+// The operand kinds every lean kernel addresses alike: the accumulator (alo / ahi), a spill register (reg_s: this
+// thread's column of the register file, 8-byte slots [reg][k][thread]) and a scalar.  A kernel's context derives from
+// this and adds its staged and direct operands.
+struct LeanRegs {
+  unsigned reg_s;
+  unsigned alo[LV], ahi[LV];
+
+  template <class F> __device__ __forceinline__ void fetch_acc(F (&out)[LV]) const {
+#pragma unroll
+    for (int k = 0; k < LV; ++k) out[k] = LAcc<F>::get(alo[k], ahi[k]);
+  }
+  template <class F> __device__ __forceinline__ void fetch_reg(int reg, F (&out)[LV]) const {
+    const unsigned addr = reg_s + (unsigned)reg * (LV * kThreads * 8);
+#pragma unroll
+    for (int k = 0; k < LV; ++k) out[k] = lean_lds<F>(addr + k * kThreads * 8);
+  }
+  template <class F> __device__ __forceinline__ void fetch_scal(u64 bits, F (&out)[LV]) const {
+    const F s = scal_as<F>(bits);
+#pragma unroll
+    for (int k = 0; k < LV; ++k) out[k] = s;
+  }
+  template <class F> __device__ __forceinline__ void store_reg(int reg, const F (&r)[LV]) const {
+    const unsigned addr = reg_s + (unsigned)reg * (LV * kThreads * 8);
+#pragma unroll
+    for (int k = 0; k < LV; ++k) lean_sts<F>(addr + k * kThreads * 8, r[k]);
+  }
+};
 
 template <class F> struct LOther;
 template <> struct LOther<double> { typedef float type; };

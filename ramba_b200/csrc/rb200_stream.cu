@@ -32,32 +32,33 @@
 
 namespace rb200 {
 
-struct StreamCtx {
+// element k of this thread in a staged tile of N * 256 elements of 4 (f32) or 8 bytes starting at `tile_s`
+template <class F, int N> __device__ __forceinline__ void stream_lds(unsigned tile_s, unsigned tid, bool f32, F (&out)[N]) {
+  if (f32) {
+    const unsigned addr = tile_s + tid * 4u;
+#pragma unroll
+    for (int k = 0; k < N; ++k) out[k] = (F)lean_lds<float>(addr + k * kThreads * 4);
+  } else {
+    const unsigned addr = tile_s + tid * 8u;
+#pragma unroll
+    for (int k = 0; k < N; ++k) out[k] = (F)lean_lds<double>(addr + k * kThreads * 8);
+  }
+}
+
+struct StreamCtx : LeanRegs {
   const StreamParams& P;
   unsigned stage_s;  // shared-window address of the current stage
-  unsigned reg_s;    // this thread's column of the register file
   unsigned tid;
   bool staged_ok;    // the current tile was staged (false: ragged last tile, read directly)
   long long row, e0; // row (mode 1, else 0); element / column of k = 0
   unsigned valid;
-  unsigned alo[LV], ahi[LV];
   double racc[RB200_MAX_REDS];  // mode 0: reduction slots
   double cacc[LV];              // mode 1: column accumulators
   __device__ __forceinline__ StreamCtx(const StreamParams& p) : P(p) {}
 
   template <class F> __device__ __forceinline__ void fetch_direct(int arg, F (&out)[LV]) {
     const LDirect& v = P.direct[arg];
-    const long long off = row * v.s1 + e0 * v.s2;
-    const long long step = (long long)kThreads * v.s2;
-    if (v.dtype == RB200_F32) {
-      const float* p = reinterpret_cast<const float*>(v.base) + off;
-#pragma unroll
-      for (int k = 0; k < LV; ++k, p += step) out[k] = ((valid >> k) & 1u) ? (F)ldg<float>(p) : F(0);
-    } else {
-      const double* p = reinterpret_cast<const double*>(v.base) + off;
-#pragma unroll
-      for (int k = 0; k < LV; ++k, p += step) out[k] = ((valid >> k) & 1u) ? (F)ldg<double>(p) : F(0);
-    }
+    ldirect_load<F, LV>(v, row * v.s1 + e0 * v.s2, (long long)kThreads * v.s2, valid, out);
   }
   template <class F> __device__ __forceinline__ void fetch(int kind, int arg, F (&out)[LV]) {
     switch (kind) {
@@ -67,54 +68,18 @@ struct StreamCtx {
           fetch_direct<F>(sv.dview, out);
           break;
         }
-        if (sv.es == 4) {
-          const unsigned addr = stage_s + sv.off + tid * 4u;
-#pragma unroll
-          for (int k = 0; k < LV; ++k) out[k] = (F)lean_lds<float>(addr + k * kThreads * 4);
-        } else {
-          const unsigned addr = stage_s + sv.off + tid * 8u;
-#pragma unroll
-          for (int k = 0; k < LV; ++k) out[k] = (F)lean_lds<double>(addr + k * kThreads * 8);
-        }
+        stream_lds<F, LV>(stage_s + sv.off, tid, sv.es == 4, out);
       } break;
       case L_DIRECT: fetch_direct<F>(arg, out); break;
-      case L_REG: {
-        const unsigned addr = reg_s + (unsigned)arg * (LV * kThreads * 8);
-#pragma unroll
-        for (int k = 0; k < LV; ++k) out[k] = lean_lds<F>(addr + k * kThreads * 8);
-      } break;
-      case L_SCAL: {
-        const u64 bits = P.scal[arg];
-        const F s = sizeof(F) == 8 ? (F)__longlong_as_double((long long)bits) : (F)__uint_as_float((unsigned)bits);
-#pragma unroll
-        for (int k = 0; k < LV; ++k) out[k] = s;
-      } break;
-      default:
-#pragma unroll
-        for (int k = 0; k < LV; ++k) out[k] = LAcc<F>::get(alo[k], ahi[k]);
+      case L_REG: fetch_reg<F>(arg, out); break;
+      case L_SCAL: fetch_scal<F>(P.scal[arg], out); break;
+      default: fetch_acc<F>(out);
     }
   }
   template <class F> __device__ __forceinline__ int chain_fetch(int, F (&)[LV]) { return 0; }  // (no chains in this kernel)
-  template <class F> __device__ __forceinline__ void store_reg(int reg, const F (&r)[LV]) {
-    const unsigned addr = reg_s + (unsigned)reg * (LV * kThreads * 8);
-#pragma unroll
-    for (int k = 0; k < LV; ++k) lean_sts<F>(addr + k * kThreads * 8, r[k]);
-  }
   template <class F> __device__ __forceinline__ void store_view(int arg, const F (&r)[LV]) {
     const LDirect& v = P.direct[arg];
-    const long long off = row * v.s1 + e0 * v.s2;
-    const long long step = (long long)kThreads * v.s2;
-    if (v.dtype == RB200_F32) {
-      float* p = reinterpret_cast<float*>(v.base) + off;
-#pragma unroll
-      for (int k = 0; k < LV; ++k, p += step)
-        if ((valid >> k) & 1u) stg<float>(p, (float)r[k]);
-    } else {
-      double* p = reinterpret_cast<double*>(v.base) + off;
-#pragma unroll
-      for (int k = 0; k < LV; ++k, p += step)
-        if ((valid >> k) & 1u) stg<double>(p, (double)r[k]);
-    }
+    ldirect_store<F, LV>(v, row * v.s1 + e0 * v.s2, (long long)kThreads * v.s2, valid, r);
   }
   template <class F> __device__ __forceinline__ void reduce(int slot, int rop, const F (&a)[LV]) {
     if constexpr (sizeof(F) == 8) {
@@ -352,42 +317,17 @@ __device__ __forceinline__ void sterm_fetch(const StreamParams& P, const STermCt
   if (t.xkind == X_STAGED) {
     const StreamStaged& sv = P.staged[t.xidx];
     if (cx.staged_ok) {
-      if (sv.es == 4) {
-        const unsigned addr = cx.stage_s + sv.off + cx.tid * 4u;
-#pragma unroll
-        for (int k = 0; k < TV; ++k) x[k] = (F)lean_lds<float>(addr + k * kThreads * 4);
-      } else {
-        const unsigned addr = cx.stage_s + sv.off + cx.tid * 8u;
-#pragma unroll
-        for (int k = 0; k < TV; ++k) x[k] = (F)lean_lds<double>(addr + k * kThreads * 8);
-      }
+      stream_lds<F, TV>(cx.stage_s + sv.off, cx.tid, sv.es == 4, x);
       return;
     }
     dview = sv.dview;  // ragged last tile: read directly
   } else if (t.xkind == X_HOIST) {
     // row-broadcast operand: this CTA's columns were copied to shared memory once
-    const unsigned base = cx.hoist_s + (unsigned)t.xidx * (TV * kThreads * 8);
-    if (P.direct[P.thoist_direct[t.xidx]].dtype == RB200_F32) {
-#pragma unroll
-      for (int k = 0; k < TV; ++k) x[k] = (F)lean_lds<float>(base + cx.tid * 4u + k * kThreads * 4);
-    } else {
-#pragma unroll
-      for (int k = 0; k < TV; ++k) x[k] = (F)lean_lds<double>(base + cx.tid * 8u + k * kThreads * 8);
-    }
+    stream_lds<F, TV>(cx.hoist_s + (unsigned)t.xidx * (TV * kThreads * 8), cx.tid, P.direct[P.thoist_direct[t.xidx]].dtype == RB200_F32, x);
     return;
   }
   const LDirect& v = P.direct[dview];
-  const long long off = cx.row * v.s1 + cx.e0 * v.s2;
-  const long long step = (long long)kThreads * v.s2;
-  if (v.dtype == RB200_F32) {
-    const float* p = reinterpret_cast<const float*>(v.base) + off;
-#pragma unroll
-    for (int k = 0; k < TV; ++k, p += step) x[k] = ((cx.valid >> k) & 1u) ? (F)ldg<float>(p) : F(0);
-  } else {
-    const double* p = reinterpret_cast<const double*>(v.base) + off;
-#pragma unroll
-    for (int k = 0; k < TV; ++k, p += step) x[k] = ((cx.valid >> k) & 1u) ? (F)ldg<double>(p) : F(0);
-  }
+  ldirect_load<F, TV>(v, cx.row * v.s1 + cx.e0 * v.s2, (long long)kThreads * v.s2, cx.valid, x);
 }
 
 template <int TV, class F> __device__ __forceinline__ void sterm_store(const StreamParams& P, const STermCtx<TV>& cx, int dview, const F (&acc)[TV]) {
@@ -489,10 +429,7 @@ __device__ __forceinline__ void sterm_step(const StreamParams& P, const STermCtx
       return;
     }
     F w = F(0);
-    if (t.flags & TF_W) {
-      const u64 sbits = P.scal[t.sidx];
-      w = sizeof(F) == 8 ? (F)__longlong_as_double((long long)sbits) : (F)__uint_as_float((unsigned)sbits);
-    }
+    if (t.flags & TF_W) w = scal_as<F>(P.scal[t.sidx]);
     if (t.kind == TK_SET) {  // straight into the running value
       if (t.xkind != X_NONE) {
         sterm_fetch<TV, F>(P, cx, t, acc);

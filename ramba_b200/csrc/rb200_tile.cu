@@ -47,16 +47,45 @@ __device__ __forceinline__ void cp_async_mbar_arrive(unsigned mbar) {
   asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(mbar) : "memory");
 }
 
-template <class TE> struct TileCtx {
+// ask for plane `pz` (halo coordinates) of the staged group into ring slot `slot`
+template <class TE>
+__device__ __forceinline__ void tile_request(const TileParams& P, const CUtensorMap* tmap, unsigned smem_s, unsigned mbar_s, unsigned slot, long long x0,
+                                             long long y0, long long pz, unsigned tid) {
+  const unsigned bar = mbar_s + 8u * slot;
+  const unsigned dst = smem_s + slot * P.plane_bytes;
+  if (P.use_tma) {
+    if (tid == 0) {
+      mbar_expect_tx(bar, (unsigned)(kTilePX * P.PY * (int)sizeof(TE)));
+      tma_load_3d(dst, tmap, (int)x0 + P.tma_shift, (int)y0, (int)pz, bar);
+    }
+  } else {
+    // rows of the box by warps, elements by lanes; out-of-range elements are zero-filled
+    const int lane = (int)(tid & 31u), warp = (int)(tid >> 5);
+    const long long Xh = P.X + P.hx, Yh = P.Y + P.hy, Zh = P.Z + P.hz;
+    for (int py = warp; py < P.PY; py += kThreads / 32) {
+      const long long gy = y0 + py;
+      const TE* row = reinterpret_cast<const TE*>(P.gcorner) + pz * P.gs0 + gy * P.gs1 + x0;
+      const unsigned drow = dst + (unsigned)(py * kTilePX * (int)sizeof(TE));
+      const bool row_ok = gy < Yh && pz >= 0 && pz < Zh;
+      for (int px = lane; px < kTilePX; px += 32) {
+        const TE* src = row + px;
+        const bool ok = row_ok && (x0 + px) < Xh && (const char*)src >= P.safe_lo && (const char*)(src + 1) <= P.safe_hi;
+        if constexpr (sizeof(TE) == 8) cp_async8(drow + px * 8u, ok ? (const void*)src : (const void*)P.safe_lo, ok);
+        else cp_async4(drow + px * 4u, ok ? (const void*)src : (const void*)P.safe_lo, ok);
+      }
+    }
+    cp_async_mbar_arrive(bar);
+  }
+}
+
+template <class TE> struct TileCtx : LeanRegs {
   const TileParams& P;
   unsigned ring_s;  // shared-window address of the plane ring
-  unsigned reg_s;   // this thread's column of the spill-register file ([reg][k][thread], 8-byte slots)
   unsigned tb0;     // byte offset of this thread's element k = 0 inside a plane, before the operand's own (dy, dx) offset
   static constexpr unsigned kstep = (unsigned)(kTileRY * kTilePX * sizeof(TE));  // byte step between elements k and k+1 inside a plane
   int fb;           // ring slot holding plane (z - hz_lo)
   long long z, gy0, gx;
   unsigned valid;
-  unsigned alo[LV], ahi[LV];
   __device__ __forceinline__ TileCtx(const TileParams& p) : P(p) {}
 
   template <class F> __device__ __forceinline__ void fetch(int kind, int arg, F (&out)[LV]) {
@@ -71,32 +100,11 @@ template <class TE> struct TileCtx {
       } break;
       case L_DIRECT: {
         const LDirect& v = P.direct[arg];
-        const long long off = z * v.s0 + gy0 * v.s1 + gx * v.s2;
-        const long long step = (long long)kTileRY * v.s1;
-        if (v.dtype == RB200_F32) {
-          const float* p = reinterpret_cast<const float*>(v.base) + off;
-#pragma unroll
-          for (int k = 0; k < LV; ++k, p += step) out[k] = ((valid >> k) & 1u) ? (F)ldg<float>(p) : F(0);
-        } else {
-          const double* p = reinterpret_cast<const double*>(v.base) + off;
-#pragma unroll
-          for (int k = 0; k < LV; ++k, p += step) out[k] = ((valid >> k) & 1u) ? (F)ldg<double>(p) : F(0);
-        }
+        ldirect_load<F, LV>(v, z * v.s0 + gy0 * v.s1 + gx * v.s2, (long long)kTileRY * v.s1, valid, out);
       } break;
-      case L_REG: {
-        const unsigned addr = reg_s + (unsigned)arg * (LV * kThreads * 8);
-#pragma unroll
-        for (int k = 0; k < LV; ++k) out[k] = lean_lds<F>(addr + k * kThreads * 8);
-      } break;
-      case L_SCAL: {
-        const u64 bits = P.scal[arg];
-        const F s = sizeof(F) == 8 ? (F)__longlong_as_double((long long)bits) : (F)__uint_as_float((unsigned)bits);
-#pragma unroll
-        for (int k = 0; k < LV; ++k) out[k] = s;
-      } break;
-      default:  // L_ACC
-#pragma unroll
-        for (int k = 0; k < LV; ++k) out[k] = LAcc<F>::get(alo[k], ahi[k]);
+      case L_REG: fetch_reg<F>(arg, out); break;
+      case L_SCAL: fetch_scal<F>(P.scal[arg], out); break;
+      default: fetch_acc<F>(out);  // L_ACC
     }
   }
   template <class F> __device__ __forceinline__ int chain_fetch(int step, F (&out)[LV]) {
@@ -109,26 +117,9 @@ template <class TE> struct TileCtx {
     for (int k = 0; k < LV; ++k) out[k] = (F)lean_lds<TE>(addr + k * kstep);
     return cs.op;
   }
-  template <class F> __device__ __forceinline__ void store_reg(int reg, const F (&r)[LV]) {
-    const unsigned addr = reg_s + (unsigned)reg * (LV * kThreads * 8);
-#pragma unroll
-    for (int k = 0; k < LV; ++k) lean_sts<F>(addr + k * kThreads * 8, r[k]);
-  }
   template <class F> __device__ __forceinline__ void store_view(int arg, const F (&r)[LV]) {
     const LDirect& v = P.direct[arg];
-    const long long off = z * v.s0 + gy0 * v.s1 + gx * v.s2;
-    const long long step = (long long)kTileRY * v.s1;
-    if (v.dtype == RB200_F32) {
-      float* p = reinterpret_cast<float*>(v.base) + off;
-#pragma unroll
-      for (int k = 0; k < LV; ++k, p += step)
-        if ((valid >> k) & 1u) stg<float>(p, (float)r[k]);
-    } else {
-      double* p = reinterpret_cast<double*>(v.base) + off;
-#pragma unroll
-      for (int k = 0; k < LV; ++k, p += step)
-        if ((valid >> k) & 1u) stg<double>(p, (double)r[k]);
-    }
+    ldirect_store<F, LV>(v, z * v.s0 + gy0 * v.s1 + gx * v.s2, (long long)kTileRY * v.s1, valid, r);
   }
   template <class F> __device__ __forceinline__ void reduce(int, int, const F (&)[LV]) {}  // (no reductions in this kernel)
 };
@@ -178,32 +169,7 @@ __global__ void __launch_bounds__(kThreads, 2) stencil_tile_kernel(const __grid_
 
     // request plane `pz` of the group (pz in halo coordinates: 0 = iteration z - hz_lo of z = 0)
     auto request = [&](long long pz) {
-      const unsigned slot = fills % (unsigned)P.D;
-      const unsigned bar = mbar_s + 8u * slot;
-      const unsigned dst = smem_s + slot * P.plane_bytes;
-      if (P.use_tma) {
-        if (tid == 0) {
-          mbar_expect_tx(bar, (unsigned)(kTilePX * P.PY * (int)sizeof(TE)));
-          tma_load_3d(dst, &tmap, (int)x0 + P.tma_shift, (int)y0, (int)pz, bar);
-        }
-      } else {
-        // rows of the box by warps, elements by lanes; out-of-range elements are zero-filled
-        const int lane = (int)(tid & 31u), warp = (int)(tid >> 5);
-        const long long Xh = P.X + P.hx, Yh = P.Y + P.hy, Zh = P.Z + P.hz;
-        for (int py = warp; py < P.PY; py += kThreads / 32) {
-          const long long gy = y0 + py;
-          const TE* row = reinterpret_cast<const TE*>(P.gcorner) + pz * P.gs0 + gy * P.gs1 + x0;
-          const unsigned drow = dst + (unsigned)(py * kTilePX * (int)sizeof(TE));
-          const bool row_ok = gy < Yh && pz >= 0 && pz < Zh;
-          for (int px = lane; px < kTilePX; px += 32) {
-            const TE* src = row + px;
-            const bool ok = row_ok && (x0 + px) < Xh && (const char*)src >= P.safe_lo && (const char*)(src + 1) <= P.safe_hi;
-            if constexpr (sizeof(TE) == 8) cp_async8(drow + px * 8u, ok ? (const void*)src : (const void*)P.safe_lo, ok);
-            else cp_async4(drow + px * 4u, ok ? (const void*)src : (const void*)P.safe_lo, ok);
-          }
-        }
-        cp_async_mbar_arrive(bar);
-      }
+      tile_request<TE>(P, &tmap, smem_s, mbar_s, fills % (unsigned)P.D, x0, y0, pz, tid);
       ++fills;
     };
 
@@ -238,37 +204,6 @@ __global__ void __launch_bounds__(kThreads, 2) stencil_tile_kernel(const __grid_
 
 
 // ---------------------------------------------------------------------------------------------
-// shared by both kernels: ask for plane `pz` (halo coordinates) of the staged group into ring slot `slot`
-template <class TE>
-__device__ __forceinline__ void tile_request(const TileParams& P, const CUtensorMap* tmap, unsigned smem_s, unsigned mbar_s, unsigned slot, long long x0,
-                                             long long y0, long long pz, unsigned tid) {
-  const unsigned bar = mbar_s + 8u * slot;
-  const unsigned dst = smem_s + slot * P.plane_bytes;
-  if (P.use_tma) {
-    if (tid == 0) {
-      mbar_expect_tx(bar, (unsigned)(kTilePX * P.PY * (int)sizeof(TE)));
-      tma_load_3d(dst, tmap, (int)x0 + P.tma_shift, (int)y0, (int)pz, bar);
-    }
-  } else {
-    // rows of the box by warps, elements by lanes; out-of-range elements are zero-filled
-    const int lane = (int)(tid & 31u), warp = (int)(tid >> 5);
-    const long long Xh = P.X + P.hx, Yh = P.Y + P.hy, Zh = P.Z + P.hz;
-    for (int py = warp; py < P.PY; py += kThreads / 32) {
-      const long long gy = y0 + py;
-      const TE* row = reinterpret_cast<const TE*>(P.gcorner) + pz * P.gs0 + gy * P.gs1 + x0;
-      const unsigned drow = dst + (unsigned)(py * kTilePX * (int)sizeof(TE));
-      const bool row_ok = gy < Yh && pz >= 0 && pz < Zh;
-      for (int px = lane; px < kTilePX; px += 32) {
-        const TE* src = row + px;
-        const bool ok = row_ok && (x0 + px) < Xh && (const char*)src >= P.safe_lo && (const char*)(src + 1) <= P.safe_hi;
-        if constexpr (sizeof(TE) == 8) cp_async8(drow + px * 8u, ok ? (const void*)src : (const void*)P.safe_lo, ok);
-        else cp_async4(drow + px * 4u, ok ? (const void*)src : (const void*)P.safe_lo, ok);
-      }
-    }
-    cp_async_mbar_arrive(bar);
-  }
-}
-
 template <class TE, int TV> struct TermCtx {
   unsigned tb0;      // byte offset of element k = 0 of this thread inside a plane
   unsigned table_s;  // shared-window address of the per-plane operand table (one 32-bit plane address per term)
@@ -285,17 +220,7 @@ __device__ __forceinline__ void term_fetch(const TileParams& P, const TermCtx<TE
     for (int k = 0; k < TV; ++k) x[k] = (F)lean_lds<TE>(addr + k * kstep);
   } else {
     const LDirect& v = P.direct[t.xidx];
-    const long long off = cx.z * v.s0 + cx.gy0 * v.s1 + cx.gx * v.s2;
-    const long long step = (long long)kTileRY * v.s1;
-    if (v.dtype == RB200_F32) {
-      const float* p = reinterpret_cast<const float*>(v.base) + off;
-#pragma unroll
-      for (int k = 0; k < TV; ++k, p += step) x[k] = ((cx.valid >> k) & 1u) ? (F)ldg<float>(p) : F(0);
-    } else {
-      const double* p = reinterpret_cast<const double*>(v.base) + off;
-#pragma unroll
-      for (int k = 0; k < TV; ++k, p += step) x[k] = ((cx.valid >> k) & 1u) ? (F)ldg<double>(p) : F(0);
-    }
+    ldirect_load<F, TV>(v, cx.z * v.s0 + cx.gy0 * v.s1 + cx.gx * v.s2, (long long)kTileRY * v.s1, cx.valid, x);
   }
 }
 
@@ -339,14 +264,12 @@ __device__ __forceinline__ void term_steps(const TileParams& P, const TermCtx<TE
     if (t.xkind != X_NONE) {
       term_fetch<TE, TV, F>(P, cx, t, s, p);
       if (t.flags & TF_W) {
-        const u64 sbits = P.scal[t.sidx];
-        const F w = sizeof(F) == 8 ? (F)__longlong_as_double((long long)sbits) : (F)__uint_as_float((unsigned)sbits);
+        const F w = scal_as<F>(P.scal[t.sidx]);
 #pragma unroll
         for (int k = 0; k < TV; ++k) p[k] = l_mul<F>(p[k], w);
       }
     } else {
-      const u64 sbits = P.scal[t.sidx];
-      const F w = sizeof(F) == 8 ? (F)__longlong_as_double((long long)sbits) : (F)__uint_as_float((unsigned)sbits);
+      const F w = scal_as<F>(P.scal[t.sidx]);
 #pragma unroll
       for (int k = 0; k < TV; ++k) p[k] = w;
     }
@@ -369,31 +292,6 @@ __device__ __forceinline__ void term_steps(const TileParams& P, const TermCtx<TE
       for (int k = 0; k < TV; ++k) acc[k] = p[k];
     }
     ++s;
-  }
-}
-
-// store the thread's TV results: `p` = address of element k = 0 in the output view, `step` = bytes between elements k and k+1
-template <int TV, class F>
-__device__ __forceinline__ void term_store(char* p, long long step, int dtype, unsigned valid, const F (&acc)[TV]) {
-  const bool full = valid == (TV == 32 ? 0xffffffffu : (1u << TV) - 1u);
-  if (dtype == RB200_F32) {
-    if (full) {
-#pragma unroll
-      for (int k = 0; k < TV; ++k, p += step) stg<float>(reinterpret_cast<float*>(p), (float)acc[k]);
-    } else {
-#pragma unroll
-      for (int k = 0; k < TV; ++k, p += step)
-        if ((valid >> k) & 1u) stg<float>(reinterpret_cast<float*>(p), (float)acc[k]);
-    }
-  } else {
-    if (full) {
-#pragma unroll
-      for (int k = 0; k < TV; ++k, p += step) stg<double>(reinterpret_cast<double*>(p), (double)acc[k]);
-    } else {
-#pragma unroll
-      for (int k = 0; k < TV; ++k, p += step)
-        if ((valid >> k) & 1u) stg<double>(reinterpret_cast<double*>(p), (double)acc[k]);
-    }
   }
 }
 
@@ -516,21 +414,21 @@ __global__ void __launch_bounds__(kThreads, (TV == 8 && sizeof(TE) == 4) ? RB200
 #pragma unroll
               for (int k = 0; k < TV; ++k) r[k] = __dadd_rn((double)a32[k], __dmul_rn((double)lean_lds<TE>(addr + k * kstep), w));
             }
-            term_store<TV, double>(optr, ostep, ov.dtype, cx.valid, r);
+            store_bytes<double, TV>(optr, ostep, ov.dtype, cx.valid, r);
           } else if (P.n_terms > P.n32) {
             double a64[TV];
 #pragma unroll
             for (int k = 0; k < TV; ++k) a64[k] = (double)a32[k];
             term_steps<TE, TV, double>(P, cx, P.n32, P.n_terms, a64);
-            term_store<TV, double>(optr, ostep, ov.dtype, cx.valid, a64);
+            store_bytes<double, TV>(optr, ostep, ov.dtype, cx.valid, a64);
           } else {
-            term_store<TV, float>(optr, ostep, ov.dtype, cx.valid, a32);
+            store_bytes<float, TV>(optr, ostep, ov.dtype, cx.valid, a32);
           }
         }
       } else {
         double a64[TV];
         term_steps<TE, TV, double>(P, cx, 0, P.n_terms, a64);
-        term_store<TV, double>(optr, ostep, ov.dtype, cx.valid, a64);
+        store_bytes<double, TV>(optr, ostep, ov.dtype, cx.valid, a64);
       }
       optr += oplane;
     }
