@@ -7,6 +7,16 @@ instantiation of the 1-D general interpreter, against two roofs for its traffic,
   roof_1r3w  the same traffic without a transcendental, `B = A*1.5; C = A*2.5; D = A*3.5` (must plan as
              kernel=stream, the streaming kernel): the best 1-read / 3-write rate the library reaches
   copy       torch's copy of 8 bytes x n (1 read / 1 write), a reference from outside the library
+  lean_walk  the chain with RB200_NO_CTA_PER_TILE=1: the lean kernel on a persistent grid walking tiles b, b+grid, ...
+             instead of one CTA per tile (plans without `grid=cta_per_tile`)
+
+What the store form can gain on this traffic was measured with benchmarks/hbm_mix.py (DESIGN §8 item 4): with the
+library's layout (2 CTAs/SM walking 2048-element tiles, A staged by bulk copies), 16-byte shuffled stores, bulk
+shared -> global stores, contiguous per-CTA tile ranges and 1 or 3 CTAs/SM all write 1R:3W within 0.3 % of plain 8-byte
+stores (11.33-11.36 ms for 1e9 float64 elements on an H100 80GB HBM3, 700 W, 1980 MHz).  That is the roof `roof_1r3w`
+stands for with the walking grid.  What moved the rate in that probe was the grid: the same work issued as one CTA per
+tile, with at most 2 CTAs resident per SM, took 10.84 ms.  The lean interpreter now runs one CTA per tile (`lean`,
+against `lean_walk`); the streaming kernel keeps its walk, which was faster for it.
 
 Every arm runs in its own process: the library reads its kill switches once per process, and the arrays of one arm
 (A, B, C, D and the previous step's outputs) are gone before the next starts.  Kernel times are CUDA events around
@@ -22,7 +32,7 @@ import subprocess
 import sys
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
-ARMS = ("full", "lean", "roof_1r3w", "copy")
+ARMS = ("full", "lean", "roof_1r3w", "copy", "lean_walk")
 
 
 def card(dev):
@@ -90,11 +100,12 @@ def run_arm(arm, n, steps, warmup):
         events, RT.profile_events = RT.profile_events, None
         ms = [a.elapsed_time(b) for a, b, _ in events]
         res = {"plan": plans, "bytes_per_element": 32, "launches_per_step": len(ms) / steps}
+        assert all(("grid=cta_per_tile" in p) == (arm == "lean") for p in plans), plans
         if arm == "roof_1r3w":
-            assert all(p.startswith("kernel=stream") for p in plans), plans
+            assert all(p.startswith("kernel=stream ") for p in plans), plans
         else:
             assert all(p.startswith("kernel=general_interpreter form=elementwise") for p in plans), plans
-            assert all(("variant=lean" in p) == (arm == "lean") for p in plans), plans
+            assert all(("variant=lean" in p) == (arm != "full") for p in plans), plans
             d = out[2][0:4096].asarray()
             import numpy as np
 
@@ -122,8 +133,11 @@ def main():
         assert arm in ARMS, arm
         env = dict(os.environ)
         env.pop("RB200_NO_LEAN_INTERP", None)
+        env.pop("RB200_NO_CTA_PER_TILE", None)
         if arm == "full":
             env["RB200_NO_LEAN_INTERP"] = "1"
+        if arm == "lean_walk":
+            env["RB200_NO_CTA_PER_TILE"] = "1"
         cmd = [sys.executable, os.path.abspath(__file__), "--arm", arm, "--n", str(args.n), "--steps", str(args.steps), "--warmup", str(args.warmup)]
         subprocess.run(cmd, env=env, check=True)
 

@@ -83,15 +83,17 @@ static int need_device(int* sms) {
 }
 
 // ---- debugging aids (A/B measurements, bisecting a parity failure), read once: each takes a kernel family, the TMA
-// loader or the row tiling out of the selection, in the launch and in rb200_describe_plan alike
+// loader, the row tiling or the lean kernel's grid of one CTA per tile out of the selection, in the launch and in
+// rb200_describe_plan alike
 struct KillSwitches {
-  bool no_tile, no_stream, no_mapred, no_terms, no_tma, no_row_mode, no_rng, no_lean;
+  bool no_tile, no_stream, no_mapred, no_terms, no_tma, no_row_mode, no_rng, no_lean, no_cta_per_tile;
 };
 static const KillSwitches& kill_switches() {
   static const KillSwitches k = {getenv("RB200_NO_TILE_KERNEL") != nullptr,   getenv("RB200_NO_STREAM_KERNEL") != nullptr,
                                  getenv("RB200_NO_MAPRED_KERNEL") != nullptr, getenv("RB200_NO_TERMS_KERNEL") != nullptr,
                                  getenv("RB200_NO_TMA") != nullptr,           getenv("RB200_NO_ROW_MODE") != nullptr,
-                                 getenv("RB200_NO_RNG") != nullptr,           getenv("RB200_NO_LEAN_INTERP") != nullptr};
+                                 getenv("RB200_NO_RNG") != nullptr,           getenv("RB200_NO_LEAN_INTERP") != nullptr,
+                                 getenv("RB200_NO_CTA_PER_TILE") != nullptr};
   return k;
 }
 
@@ -230,7 +232,7 @@ static void make_plan(const rb200_fused_op* op, int sms, Plan& pl) {
     return;
   }
   // ---- the general interpreter
-  plan_interp(op, sms, !ks.no_row_mode, !ks.no_lean, pl.interp);
+  plan_interp(op, sms, !ks.no_row_mode, !ks.no_lean, !ks.no_cta_per_tile, pl.interp);
   pl.form = FORM_INTERP;
   pl.n_written = pl.interp.n_written;
 }

@@ -22,12 +22,14 @@ struct InterpPlan {
   InterpForm form;
   KParams k;
   bool lean;  // INTERP_ELEMENTWISE, 1-D: the lean instantiation (handler ids are lean ids)
+  bool per_tile;  // the lean kernel runs one CTA per tile instead of a persistent grid walking the tiles
   long long blocks;
   size_t smem;
   int n_written;
 };
-// any valid, non-empty op list.  row_mode / lean: the N-d row tiling and the lean 1-D kernel may be chosen
-void plan_interp(const rb200_fused_op* op, int sms, bool row_mode, bool lean, InterpPlan& I);
+// any valid, non-empty op list.  row_mode / lean / per_tile: the N-d row tiling, the lean 1-D kernel and its grid of
+// one CTA per tile may be chosen
+void plan_interp(const rb200_fused_op* op, int sms, bool row_mode, bool lean, bool per_tile, InterpPlan& I);
 // one line for rb200_describe_plan
 std::string describe_interp(const rb200_fused_op* op, const InterpPlan& I);
 
