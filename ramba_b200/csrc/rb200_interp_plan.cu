@@ -3,6 +3,8 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <string>
+
 #include "rb200_handlers.h"
 #include "rb200_launch.h"
 #include "rb200_plan.h"
@@ -296,9 +298,16 @@ std::string describe_interp(const rb200_fused_op* op, const InterpPlan& pl) {
   const char* form = pl.form == INTERP_ELEMENTWISE ? "elementwise" : pl.form == INTERP_AXIS_AS_1D ? "axis_as_1d" : "axis_reduce";
   const char* tiling = pl.form != INTERP_ELEMENTWISE || op->ndim == 1 ? "" : pl.k.row_chunks > 0 ? " tiling=row" : " tiling=flat";
   char buf[220];
-  snprintf(buf, sizeof(buf), "kernel=general_interpreter form=%s ndim=%d insns=%d views=%d%s ctas=%lld%s smem=%zu%s", form, op->ndim, op->n_insns,
-           op->n_views, tiling, pl.blocks, pl.per_tile ? " grid=cta_per_tile" : "", pl.smem, pl.lean ? " variant=lean" : "");
-  return buf;
+  snprintf(buf, sizeof(buf), "kernel=general_interpreter form=%s ndim=%d insns=%d views=%d%s ctas=%lld%s smem=%zu", form, op->ndim, op->n_insns,
+           op->n_views, tiling, pl.blocks, pl.per_tile ? " grid=cta_per_tile" : "", pl.smem);
+  std::string s = buf;
+  // the instructions (by index) without a specialised handler, which take the generic decode path (the axis kernel runs
+  // every instruction on it)
+  if (pl.form != INTERP_AXIS_REDUCE)
+    for (int i = 0, n = 0; i < pl.k.n_insns; ++i)
+      if (pl.k.handler[i] == H_GENERIC) s += (n++ ? "," : " generic=") + std::to_string(i);
+  if (pl.lean) s += " variant=lean";
+  return s;
 }
 
 }  // namespace rb200

@@ -266,9 +266,11 @@ __device__ __forceinline__ void store_view(char* base, int dtype, const long lon
 // ---------------------------------------------------------------------------------------------
 // fp64 sin/cos for V elements in lockstep (shared constants, no per-element branches):
 // Cody-Waite reduction with a 3-part pi/2 and FMAs (j = rint(x*2/pi) by the 1.5*2^52 trick, exact
-// for |x| < 2^31*pi/2), fdlibm kernel polynomials on [-pi/4, pi/4], quadrant select.  Measured
-// against 200-bit references: <= 1.31 ulp on [0, 1e6] and +-1e9.  Anything larger (or NaN/Inf) takes
-// the CUDA library routine.
+// for |x| < 2^31*pi/2), fdlibm kernel polynomials on [-pi/4, pi/4], quadrant select.  Against 200-bit
+// references: at most 1.513 ulp on an H100 (tests/test_sincos_accuracy.py holds it to 1.55; the largest
+// error among 3e8 arguments below 1e9, arange * 0.001 and uniform samples).  If any of a thread's V
+// elements is 1e9 or more in magnitude, NaN or Inf, all V take the CUDA library routine (<= 2 ulp), so
+// an element's result can differ by about 1 ulp with its neighbours.
 // library routines out of line: their large-argument paths keep a table in local memory and would
 // otherwise be inlined once per element into every trigonometric handler
 static __device__ __noinline__ double2 sincos_lib(double x) {
@@ -306,15 +308,19 @@ template <int V> __device__ __forceinline__ void sincos_v(const double (&x)[V], 
     const int q = __double2loint(t);
     const double j = t - MAGIC;
     double y = fma(-j, HI, x[k]);
-    y = fma(-j, MID, y);
-    y = fma(-j, LO, y);
+    const double y2 = fma(-j, MID, y);
+    y = fma(-j, LO, y2);
     const double z = y * y;
     double ps = fma(z, S6, S5);
     ps = fma(z, ps, S4);
     ps = fma(z, ps, S3);
     ps = fma(z, ps, S2);
     ps = fma(z, ps, S1);
-    const double sy = fma(y * z, ps, y);
+    // sin(y) has the sign of y, and y that of y2 (|j * LO| < 1e-24, far below any nonzero |y2| for |x| < 1e9) - but
+    // only y2 keeps x = -0 as -0: the last step adds -j * LO = +0 (j = +0, LO < 0), and so does the polynomial
+    // (y * z * ps with ps < 0), and -0 + +0 is +0.  Taking the sign from y2 makes sin(-0) = -0 at the cost of one
+    // LOP3, without a compare or a branch.
+    const double sy = copysign(fma(y * z, ps, y), y2);
     double pc = fma(z, C6, C5);
     pc = fma(z, pc, C4);
     pc = fma(z, pc, C3);
