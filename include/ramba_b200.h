@@ -365,6 +365,33 @@ int64_t rb200_group_reduce_scratch_bytes(const rb200_index_view* src, int32_t ax
  * argument (reason in rb200_last_error); the text stays valid until the next call on this thread.                    */
 const char* rb200_describe_group_plan(const rb200_index_view* src, int32_t axis, int32_t n_groups);
 
+/* ---- first-occurrence index reductions (argmax, argmin, nanargmax, nanargmin) ------------------------------------------
+ * Every element of the view becomes an int64 order key:
+ *   - an integer: its value;
+ *   - a float: -0.0 becomes +0.0, then its bit pattern b (float32: the 32-bit pattern, sign-extended) gives
+ *     b >= 0 ? b : b ^ INT64_MAX; a NaN gives INT64_MAX for ARG_MAX and INT64_MIN for ARG_MIN;
+ *   - ARG_MIN and ARG_NANMIN then take ~key;
+ *   - ARG_NANMAX and ARG_NANMIN give a NaN element no candidate.
+ * Every op is then "the largest key, then the smallest index", a total order, so the result does not depend on the
+ * launch shape.  An output with no candidate (an empty extent, or only NaN in a nan variant) gets index INT64_MAX and
+ * key INT64_MIN.
+ * Indices are global: the caller gives origin[d], the global coordinate of the view's element (0, ..., 0), and
+ * gstride[d], the C-order strides of the global array's shape (host arrays of src->ndim entries, read during the call).
+ *   axis = RB200_ARG_ALL_AXES: one output, the flat C-order index sum((origin[d] + c_d) * gstride[d]);
+ *   axis = k: one output per kept element (C order over the view's dims without k), the position origin[k] + c_k.
+ * out_idx and out_key: device, one int64 per output.  src_dtype: RB200_F64, F32, I64 or I32 (matching
+ * src->elem_bytes).  scratch: rb200_arg_reduce_scratch_bytes() bytes (may be NULL when that is 0).  Malformed arguments
+ * are rejected with a reason before any device query.                                                                */
+enum rb200_arg_op { RB200_ARG_MAX = 0, RB200_ARG_MIN = 1, RB200_ARG_NANMAX = 2, RB200_ARG_NANMIN = 3, RB200_ARG_NUM_OPS = 4 };
+#define RB200_ARG_ALL_AXES (-1)
+
+int rb200_arg_reduce(const rb200_index_view* src, int32_t src_dtype, int32_t axis, int32_t op, const int64_t* origin, const int64_t* gstride,
+                     int64_t* out_idx, int64_t* out_key, void* scratch, void* stream);
+int64_t rb200_arg_reduce_scratch_bytes(const rb200_index_view* src, int32_t axis);
+/* One text line: form (global / row / column / general), chunk, split, outputs, CTAs, scratch.  Needs no device.  NULL
+ * on a malformed argument (reason in rb200_last_error); the text stays valid until the next call on this thread.      */
+const char* rb200_describe_arg_plan(const rb200_index_view* src, int32_t axis);
+
 /* Which kernel rb200_run_deferred_ops would run `op` on and how (staged views, halos, TMA or cp.async loader, ring depth,
  * lean instructions, CTAs), as one text line in out[0..cap).  Needs no device and touches no pointer: the counterpart
  * of RAMBA_SHOW_CODE printing the generated kernel (ramba/ramba.py:8266-8284).                                       */

@@ -39,6 +39,9 @@ RED_ADD, RED_MUL, RED_MIN, RED_MAX = range(4)
 PHILOX_UNIFORM64, PHILOX_UNIFORM32, PHILOX_NORMAL64, PHILOX_INTEGER = range(4)
 # grouped-reduction ops (rb200_group_reduce)
 GROUP_SUM, GROUP_PROD, GROUP_MIN, GROUP_MAX, GROUP_NANSUM, GROUP_NANCOUNT, GROUP_SQDEV = range(7)
+# index-reduction ops (rb200_arg_reduce) and its "every axis" value of `axis`
+ARG_MAX, ARG_MIN, ARG_NANMAX, ARG_NANMIN = range(4)
+ARG_ALL_AXES = -1
 
 
 class Insn(C.Structure):
@@ -145,6 +148,9 @@ EXPORTS = [
     "rb200_group_reduce",
     "rb200_group_reduce_scratch_bytes",
     "rb200_describe_group_plan",
+    "rb200_arg_reduce",
+    "rb200_arg_reduce_scratch_bytes",
+    "rb200_describe_arg_plan",
 ]
 
 _LIB = None
@@ -210,6 +216,13 @@ def load():
     lib.rb200_group_reduce_scratch_bytes.restype = C.c_int64
     lib.rb200_describe_group_plan.argtypes = [C.POINTER(IndexView), C.c_int32, C.c_int32]
     lib.rb200_describe_group_plan.restype = C.c_char_p
+    lib.rb200_arg_reduce.argtypes = [C.POINTER(IndexView), C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_void_p]
+    lib.rb200_arg_reduce.restype = C.c_int
+    lib.rb200_arg_reduce_scratch_bytes.argtypes = [C.POINTER(IndexView), C.c_int32]
+    lib.rb200_arg_reduce_scratch_bytes.restype = C.c_int64
+    lib.rb200_describe_arg_plan.argtypes = [C.POINTER(IndexView), C.c_int32]
+    lib.rb200_describe_arg_plan.restype = C.c_char_p
     if lib.rb200_abi_version() != ABI_VERSION:
         raise CabiError("libramba_b200.so ABI %d != binding ABI %d: rebuild" % (lib.rb200_abi_version(), ABI_VERSION))
     _LIB = lib
@@ -356,3 +369,31 @@ def group_plan_fields(text):
         k, v = kv.split("=", 1)
         out[k] = int(v) if v.lstrip("-").isdigit() else v
     return out
+
+
+def arg_coords(origin, gstride):
+    """(origin, gstride) as host int64 arrays for rb200_arg_reduce (the caller keeps them alive for the call)."""
+    import numpy as np
+
+    return np.ascontiguousarray(origin, dtype=np.int64), np.ascontiguousarray(gstride, dtype=np.int64)
+
+
+def arg_reduce(view, src_dtype, axis, op, origin, gstride, out_idx, out_key, scratch, stream=None):
+    """rb200_arg_reduce; origin / gstride: host int64 arrays of view.ndim entries (see arg_coords)."""
+    check(load().rb200_arg_reduce(C.byref(view), src_dtype, axis, op, _p(origin.ctypes.data), _p(gstride.ctypes.data), _p(out_idx), _p(out_key),
+                                  _p(scratch), _p(stream)))
+
+
+def arg_reduce_scratch_bytes(view, axis):
+    n = int(load().rb200_arg_reduce_scratch_bytes(C.byref(view), axis))
+    if n < 0:
+        check(1)
+    return n
+
+
+def describe_arg_plan(view, axis):
+    """One text line: the form, chunk, split and CTAs the library would reduce this view with (no device needed)."""
+    s = load().rb200_describe_arg_plan(C.byref(view), axis)
+    if s is None:
+        check(1)
+    return s.decode()

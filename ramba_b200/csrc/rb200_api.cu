@@ -9,6 +9,7 @@
 
 #include "rb200_launch.h"
 #include "rb200_plan.h"
+#include "rb200_argred.h"
 #include "rb200_group.h"
 #include "rb200_index.h"
 #include "rb200_rng.h"
@@ -375,6 +376,17 @@ static int check_group_args(const rb200_index_view* src, int axis, int n_groups,
 
 static thread_local std::string g_group_plan_text;
 
+// ---- index reductions: argument checks (before any device query) and the plan
+static int check_arg_args(const rb200_index_view* src, int axis, ArgPlan* P) {
+  if (const int rc = check_index_view(src, "arg_reduce")) return rc;
+  if (axis != RB200_ARG_ALL_AXES && (axis < 0 || axis >= src->ndim)) return fail("arg_reduce: axis out of range");
+  make_arg_plan(*src, axis, P);
+  if (P->ctas >= (1ll << 31)) return fail("arg_reduce: too many outputs for one launch");
+  return 0;
+}
+
+static thread_local std::string g_arg_plan_text;
+
 extern "C" {
 
 const char* rb200_last_error(void) { return g_last_error.c_str(); }
@@ -513,6 +525,43 @@ int rb200_group_reduce(const rb200_index_view* src, int32_t src_dtype, int32_t a
   const cudaError_t e = launch_group(P, src_dtype, op, (const long long*)groups->offsets, (const long long*)groups->members, (const double*)center, out,
                                      scratch, (cudaStream_t)stream_v);
   if (e != cudaSuccess) return fail_cuda("group kernel launch", e);
+  g_launches.fetch_add(1);
+  return 0;
+}
+
+int64_t rb200_arg_reduce_scratch_bytes(const rb200_index_view* src, int32_t axis) {
+  ArgPlan P;
+  if (check_arg_args(src, axis, &P)) return -1;
+  return (int64_t)P.scratch_bytes;
+}
+
+const char* rb200_describe_arg_plan(const rb200_index_view* src, int32_t axis) {
+  ArgPlan P;
+  if (check_arg_args(src, axis, &P)) return nullptr;
+  char buf[200];
+  snprintf(buf, sizeof(buf), "kernel=argreduce form=%s chunk=%lld split=%d outputs=%lld ctas=%lld scratch=%lld", arg_form_name(P.form), P.C, P.S,
+           P.n_out, P.ctas, P.scratch_bytes);
+  g_arg_plan_text = buf;
+  return g_arg_plan_text.c_str();
+}
+
+int rb200_arg_reduce(const rb200_index_view* src, int32_t src_dtype, int32_t axis, int32_t op, const int64_t* origin, const int64_t* gstride,
+                     int64_t* out_idx, int64_t* out_key, void* scratch, void* stream_v) {
+  if (op < 0 || op >= RB200_ARG_NUM_OPS) return fail("arg_reduce: bad op");
+  if (src_dtype != RB200_F64 && src_dtype != RB200_F32 && src_dtype != RB200_I64 && src_dtype != RB200_I32)
+    return fail("arg_reduce: source dtype must be float64, float32, int64 or int32");
+  if (src && dtype_size(src_dtype) != src->elem_bytes) return fail("arg_reduce: elem_bytes does not match the source dtype");
+  ArgPlan P;
+  if (const int rc = check_arg_args(src, axis, &P)) return rc;
+  if (!origin || !gstride) return fail("arg_reduce: null origin or gstride");
+  if (!out_idx || !out_key) return fail("arg_reduce: null out");
+  if (P.scratch_bytes && !scratch) return fail("arg_reduce: null scratch (this plan splits the walk)");
+  if (P.n_out == 0) return 0;
+  bind_arg_coords(*src, axis, (const long long*)origin, (const long long*)gstride, &P);
+  int sms;
+  if (const int rc = need_device(&sms)) return rc;
+  const cudaError_t e = launch_arg(P, src_dtype, op, (long long*)out_idx, (long long*)out_key, scratch, (cudaStream_t)stream_v);
+  if (e != cudaSuccess) return fail_cuda("arg kernel launch", e);
   g_launches.fetch_add(1);
   return 0;
 }

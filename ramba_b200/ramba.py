@@ -26,6 +26,7 @@ import torch
 
 from . import _cabi as cabi
 from . import advindex
+from . import argreduce
 from . import blocks
 from . import common
 from . import shardview
@@ -2486,6 +2487,29 @@ def nanmean(a, axis=None, dtype=None):
 
 
 for _n in ("concatenate", "stack", "pad", "split", "rollaxis", "nansum", "nanmean"):
+    HANDLED_FUNCTIONS[_n] = globals()[_n]
+
+
+# ---- first-occurrence index reductions on the index-reduction kernel (ramba_b200/argreduce.py)
+def argmax(a, axis=None, out=None, *, keepdims=False):
+    return argreduce.arg_reduce(a, "argmax", axis, out, keepdims)
+
+
+def argmin(a, axis=None, out=None, *, keepdims=False):
+    return argreduce.arg_reduce(a, "argmin", axis, out, keepdims)
+
+
+def nanargmax(a, axis=None, out=None, *, keepdims=False):
+    return argreduce.arg_reduce(a, "nanargmax", axis, out, keepdims)
+
+
+def nanargmin(a, axis=None, out=None, *, keepdims=False):
+    return argreduce.arg_reduce(a, "nanargmin", axis, out, keepdims)
+
+
+ndarray.argmax = argmax
+ndarray.argmin = argmin
+for _n in ("argmax", "argmin", "nanargmax", "nanargmin"):
     HANDLED_FUNCTIONS[_n] = globals()[_n]
 
 

@@ -147,6 +147,14 @@ class CudaBackend:
         cabi.group_reduce(view, src_code, axis, table, op, center, out, scratch.data_ptr() if nbytes else None, self.stream_handle())
         return scratch
 
+    def arg_reduce(self, view, src_code, axis, op, origin, gstride, out_idx, out_key):
+        """rb200_arg_reduce on the current stream; returns the scratch buffer (the caller keeps it alive)."""
+        nbytes = cabi.arg_reduce_scratch_bytes(view, axis)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device) if nbytes else None
+        o, g = cabi.arg_coords(origin, gstride)
+        cabi.arg_reduce(view, src_code, axis, op, o, g, out_idx, out_key, scratch.data_ptr() if nbytes else None, self.stream_handle())
+        return scratch
+
     def init_process_group(self):
         dist.init_process_group("nccl", device_id=self.device)
 
@@ -466,6 +474,14 @@ class Runtime:
         accumulator class) receives op over the members of every group (table: a cabi.GroupTable).  Returns the scratch
         buffer (or None)."""
         scratch = self.be().group_reduce(view, src_code, axis, table, op, center, out)
+        self.launches += 1
+        return scratch
+
+    def arg_reduce(self, view, src_code, axis, op, origin, gstride, out_idx, out_key):
+        """First-occurrence index reduction of one local view through the C-ABI (rb200_arg_reduce): over every axis
+        (axis = cabi.ARG_ALL_AXES) or along one, writing global indices and order keys to the device addresses out_idx
+        and out_key; origin / gstride place the view in the global array.  Returns the scratch buffer (or None)."""
+        scratch = self.be().arg_reduce(view, src_code, axis, op, origin, gstride, out_idx, out_key)
         self.launches += 1
         return scratch
 
