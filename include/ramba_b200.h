@@ -392,6 +392,34 @@ int64_t rb200_arg_reduce_scratch_bytes(const rb200_index_view* src, int32_t axis
  * on a malformed argument (reason in rb200_last_error); the text stays valid until the next call on this thread.      */
 const char* rb200_describe_arg_plan(const rb200_index_view* src, int32_t axis);
 
+/* ---- stream compaction (nonzero, flatnonzero, extract) ---------------------------------------------------------------
+ * An element of the condition view is selected when its stored value is nonzero: bits != 0, and for float32 / float64
+ * the bits without the sign (-0.0 is not selected, NaN is).  The view's C-order positions are cut into runs of run_len
+ * positions (run_len divides the view's size: a rank's part of a C-order array is such a set of runs), and every run
+ * into chunks of at most RB200_COMPACT_CHUNK positions; chunk c of run r is number q = c * n_runs + r, with
+ * cpr = ceil(run_len / RB200_COMPACT_CHUNK) chunks per run.
+ *   rb200_compact_count writes counts[q], the selected elements of chunk q (device, n_runs * cpr int64).
+ *   rb200_compact writes the payload of every selected element of chunk q, in C order, from position
+ *     run_base[r] + incl[q] - counts[q], where incl is the inclusive scan of counts along each run (for cpr == 1, incl
+ *     may be counts itself; rb200_cumulative over [cpr][n_runs] with n_inner = n_runs gives it otherwise).
+ *   Payload forms: RB200_COMPACT_VALUES: the element of `values` (same shape as cond, 1/2/4/8-byte elements) at the
+ *     same position, out[0] elem_bytes per element; RB200_COMPACT_FLAT: sum((origin[d] + c_d) * gstride[d]), out[0] int64;
+ *     RB200_COMPACT_COORDS: origin[d] + c_d into out[d] for every dim d of the view (int64 each).
+ * cond_dtype: any storage dtype matching cond->elem_bytes.  origin / gstride: host arrays of cond->ndim entries, out: a
+ * host array of device pointers; all read during the call.  Positions depend only on the data.  No scratch.  Malformed
+ * arguments are rejected with a reason before any device query.                                                       */
+#define RB200_COMPACT_CHUNK 4096
+enum rb200_compact_form { RB200_COMPACT_VALUES = 0, RB200_COMPACT_FLAT = 1, RB200_COMPACT_COORDS = 2 };
+
+int rb200_compact_count(const rb200_index_view* cond, int32_t cond_dtype, int64_t run_len, int64_t* counts, void* stream);
+int rb200_compact(const rb200_index_view* cond, int32_t cond_dtype, int64_t run_len, const int64_t* counts, const int64_t* incl,
+                  const int64_t* run_base, int32_t form, const rb200_index_view* values, const int64_t* origin, const int64_t* gstride,
+                  void* const* out, void* stream);
+/* One text line: runs, run length, chunks per run, runs per CTA (a CTA covers one chunk or several whole short runs),
+ * CTAs, and whether the condition is read with 16-byte vector loads.  Needs no device.  NULL on a malformed argument (reason in rb200_last_error); the text stays valid until
+ * the next call on this thread.                                                                                       */
+const char* rb200_describe_compact_plan(const rb200_index_view* cond, int64_t run_len);
+
 /* Which kernel rb200_run_deferred_ops would run `op` on and how (staged views, halos, TMA or cp.async loader, ring depth,
  * lean instructions, CTAs), as one text line in out[0..cap).  Needs no device and touches no pointer: the counterpart
  * of RAMBA_SHOW_CODE printing the generated kernel (ramba/ramba.py:8266-8284).                                       */

@@ -42,6 +42,9 @@ GROUP_SUM, GROUP_PROD, GROUP_MIN, GROUP_MAX, GROUP_NANSUM, GROUP_NANCOUNT, GROUP
 # index-reduction ops (rb200_arg_reduce) and its "every axis" value of `axis`
 ARG_MAX, ARG_MIN, ARG_NANMAX, ARG_NANMIN = range(4)
 ARG_ALL_AXES = -1
+# stream-compaction payload forms (rb200_compact) and its chunk size
+COMPACT_VALUES, COMPACT_FLAT, COMPACT_COORDS = range(3)
+COMPACT_CHUNK = 4096
 
 
 class Insn(C.Structure):
@@ -151,6 +154,9 @@ EXPORTS = [
     "rb200_arg_reduce",
     "rb200_arg_reduce_scratch_bytes",
     "rb200_describe_arg_plan",
+    "rb200_compact_count",
+    "rb200_compact",
+    "rb200_describe_compact_plan",
 ]
 
 _LIB = None
@@ -223,6 +229,13 @@ def load():
     lib.rb200_arg_reduce_scratch_bytes.restype = C.c_int64
     lib.rb200_describe_arg_plan.argtypes = [C.POINTER(IndexView), C.c_int32]
     lib.rb200_describe_arg_plan.restype = C.c_char_p
+    lib.rb200_compact_count.argtypes = [C.POINTER(IndexView), C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.rb200_compact_count.restype = C.c_int
+    lib.rb200_compact.argtypes = [C.POINTER(IndexView), C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.rb200_compact.restype = C.c_int
+    lib.rb200_describe_compact_plan.argtypes = [C.POINTER(IndexView), C.c_int64]
+    lib.rb200_describe_compact_plan.restype = C.c_char_p
     if lib.rb200_abi_version() != ABI_VERSION:
         raise CabiError("libramba_b200.so ABI %d != binding ABI %d: rebuild" % (lib.rb200_abi_version(), ABI_VERSION))
     _LIB = lib
@@ -394,6 +407,30 @@ def arg_reduce_scratch_bytes(view, axis):
 def describe_arg_plan(view, axis):
     """One text line: the form, chunk, split and CTAs the library would reduce this view with (no device needed)."""
     s = load().rb200_describe_arg_plan(C.byref(view), axis)
+    if s is None:
+        check(1)
+    return s.decode()
+
+
+def compact_count(cond, cond_dtype, run_len, counts, stream=None):
+    """rb200_compact_count: counts (device int64, n_runs * chunks per run) of the selected elements of every chunk."""
+    check(load().rb200_compact_count(C.byref(cond), cond_dtype, run_len, _p(counts), _p(stream)))
+
+
+def compact(cond, cond_dtype, run_len, counts, incl, run_base, form, values, origin, gstride, outs, stream=None):
+    """rb200_compact; values: an IndexView or None; origin / gstride: host int64 arrays or None; outs: device addresses."""
+    import numpy as np
+
+    o = np.ascontiguousarray(origin if origin is not None else np.zeros(max(cond.ndim, 1)), dtype=np.int64)
+    g = np.ascontiguousarray(gstride if gstride is not None else np.zeros(max(cond.ndim, 1)), dtype=np.int64)
+    ptrs = (C.c_void_p * max(len(outs), 1))(*[C.c_void_p(x) for x in outs])
+    check(load().rb200_compact(C.byref(cond), cond_dtype, run_len, _p(counts), _p(incl), _p(run_base), form,
+                               C.byref(values) if values is not None else None, _p(o.ctypes.data), _p(g.ctypes.data), ptrs, _p(stream)))
+
+
+def describe_compact_plan(cond, run_len):
+    """One text line: runs, chunks and CTAs the library would compact this condition view with (no device needed)."""
+    s = load().rb200_describe_compact_plan(C.byref(cond), run_len)
     if s is None:
         check(1)
     return s.decode()

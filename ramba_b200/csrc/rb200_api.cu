@@ -10,6 +10,7 @@
 #include "rb200_launch.h"
 #include "rb200_plan.h"
 #include "rb200_argred.h"
+#include "rb200_compact.h"
 #include "rb200_group.h"
 #include "rb200_index.h"
 #include "rb200_rng.h"
@@ -387,6 +388,25 @@ static int check_arg_args(const rb200_index_view* src, int axis, ArgPlan* P) {
 
 static thread_local std::string g_arg_plan_text;
 
+// ---- stream compaction: argument checks (before any device query) and the plan
+static int check_compact_args(const rb200_index_view* cond, long long run_len, CompactPlan* P) {
+  if (const int rc = check_index_view(cond, "compact")) return rc;
+  make_compact_plan(*cond, run_len, P);
+  if (run_len < 1 || P->n % run_len != 0) return fail("compact: run_len must be >= 1 and divide the view's size");
+  if (P->ctas >= (1ll << 31)) return fail("compact: too many chunks for one launch");
+  return 0;
+}
+
+static int check_compact_dtype(const rb200_index_view* cond, int cond_dtype) {
+  if (cond_dtype < 0 || cond_dtype >= RB200_NUM_DTYPES) return fail("compact: bad condition dtype");
+  if (dtype_size(cond_dtype) != cond->elem_bytes) return fail("compact: elem_bytes does not match the condition dtype");
+  return 0;
+}
+
+static bool compact_is_float(int dt) { return dt == RB200_F64 || dt == RB200_F32; }
+
+static thread_local std::string g_compact_plan_text;
+
 extern "C" {
 
 const char* rb200_last_error(void) { return g_last_error.c_str(); }
@@ -562,6 +582,75 @@ int rb200_arg_reduce(const rb200_index_view* src, int32_t src_dtype, int32_t axi
   if (const int rc = need_device(&sms)) return rc;
   const cudaError_t e = launch_arg(P, src_dtype, op, (long long*)out_idx, (long long*)out_key, scratch, (cudaStream_t)stream_v);
   if (e != cudaSuccess) return fail_cuda("arg kernel launch", e);
+  g_launches.fetch_add(1);
+  return 0;
+}
+
+const char* rb200_describe_compact_plan(const rb200_index_view* cond, int64_t run_len) {
+  CompactPlan P;
+  if (check_compact_args(cond, run_len, &P)) return nullptr;
+  const bool vec = P.cond.nd == 1 && P.cond.stride[0] == 1;
+  char buf[256];
+  snprintf(buf, sizeof(buf), "kernel=compact runs=%lld run_len=%lld chunk=%d chunks_per_run=%lld runs_per_cta=%lld ctas=%lld load=%s", P.n_runs,
+           P.run_len, RB200_COMPACT_CHUNK, P.cpr, P.runs_per_cta, P.ctas, vec ? "vector" : "strided");
+  g_compact_plan_text = buf;
+  return g_compact_plan_text.c_str();
+}
+
+int rb200_compact_count(const rb200_index_view* cond, int32_t cond_dtype, int64_t run_len, int64_t* counts, void* stream_v) {
+  CompactPlan P;
+  if (const int rc = check_compact_args(cond, run_len, &P)) return rc;
+  if (const int rc = check_compact_dtype(cond, cond_dtype)) return rc;
+  if (P.n == 0) return 0;
+  if (!counts) return fail("compact_count: null counts");
+  int sms;
+  if (const int rc = need_device(&sms)) return rc;
+  const cudaError_t e = launch_compact_count(P, compact_is_float(cond_dtype), (long long*)counts, (cudaStream_t)stream_v);
+  if (e != cudaSuccess) return fail_cuda("compact count kernel launch", e);
+  g_launches.fetch_add(1);
+  return 0;
+}
+
+int rb200_compact(const rb200_index_view* cond, int32_t cond_dtype, int64_t run_len, const int64_t* counts, const int64_t* incl,
+                  const int64_t* run_base, int32_t form, const rb200_index_view* values, const int64_t* origin, const int64_t* gstride,
+                  void* const* out, void* stream_v) {
+  if (form != RB200_COMPACT_VALUES && form != RB200_COMPACT_FLAT && form != RB200_COMPACT_COORDS) return fail("compact: bad form");
+  CompactPlan P;
+  if (const int rc = check_compact_args(cond, run_len, &P)) return rc;
+  if (const int rc = check_compact_dtype(cond, cond_dtype)) return rc;
+  CompactOut O;
+  O.form = form;
+  O.k = form == RB200_COMPACT_COORDS ? cond->ndim : 1;
+  O.g0 = 0;
+  if (form == RB200_COMPACT_VALUES) {
+    if (const int rc = check_index_view(values, "compact values")) return rc;
+    if (values->ndim != cond->ndim) return fail("compact: values and condition differ in shape");
+    for (int d = 0; d < cond->ndim; ++d)
+      if (values->shape[d] != cond->shape[d]) return fail("compact: values and condition differ in shape");
+    O.values = make_compact_view(*values);
+  } else {
+    if (!origin || (form == RB200_COMPACT_FLAT && !gstride)) return fail("compact: null origin or gstride");
+    for (int d = 0; d < cond->ndim; ++d) {
+      O.cshape[d] = cond->shape[d];
+      O.origin[d] = origin[d];
+      O.gstride[d] = form == RB200_COMPACT_FLAT ? gstride[d] : 0;
+      O.g0 += O.origin[d] * O.gstride[d];
+    }
+    if (form == RB200_COMPACT_FLAT) O.k = cond->ndim;
+  }
+  if (P.n == 0) return 0;
+  if (!counts || !incl || !run_base) return fail("compact: null counts, incl or run_base");
+  if (!out) return fail("compact: null out");
+  const int n_out = form == RB200_COMPACT_COORDS ? cond->ndim : 1;
+  for (int i = 0; i < n_out; ++i) {
+    if (!out[i]) return fail("compact: null out");
+    O.out[i] = out[i];
+  }
+  int sms;
+  if (const int rc = need_device(&sms)) return rc;
+  const cudaError_t e = launch_compact(P, compact_is_float(cond_dtype), (const long long*)counts, (const long long*)incl, (const long long*)run_base, O,
+                                       (cudaStream_t)stream_v);
+  if (e != cudaSuccess) return fail_cuda("compact kernel launch", e);
   g_launches.fetch_add(1);
   return 0;
 }

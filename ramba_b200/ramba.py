@@ -27,6 +27,7 @@ import torch
 from . import _cabi as cabi
 from . import advindex
 from . import argreduce
+from . import compaction
 from . import blocks
 from . import common
 from . import shardview
@@ -2116,7 +2117,9 @@ def allclose(a, b, rtol=1e-5, atol=1e-8, equal_nan=False):
 
 
 def where(cond, a=None, b=None):
-    """`a if cond else b` as one fused statement (ramba/ramba.py:9755-9799)."""
+    """`a if cond else b` as one fused statement (ramba/ramba.py:9755-9799); with the condition alone, nonzero(cond)."""
+    if a is None and b is None:
+        return compaction.nonzero(cond)
     cond, a, b = _as_nd(cond), _as_nd(a), _as_nd(b)
     shape = cond.shape
     for x in (a, b):
@@ -2510,6 +2513,26 @@ def nanargmin(a, axis=None, out=None, *, keepdims=False):
 ndarray.argmax = argmax
 ndarray.argmin = argmin
 for _n in ("argmax", "argmin", "nanargmax", "nanargmin"):
+    HANDLED_FUNCTIONS[_n] = globals()[_n]
+
+
+# ---- stream compaction on the compaction kernel (ramba_b200/compaction.py)
+nonzero = compaction.nonzero
+flatnonzero = compaction.flatnonzero
+argwhere = compaction.argwhere
+count_nonzero = compaction.count_nonzero
+extract = compaction.extract
+
+
+def compress(condition, a, axis=None, out=None):
+    if out is not None:
+        raise NotImplementedError("compress: out= is not supported")
+    return compaction.compress(condition, a, axis)
+
+
+ndarray.nonzero = nonzero
+ndarray.compress = lambda self, condition, axis=None, out=None: compress(condition, self, axis, out)
+for _n in ("nonzero", "flatnonzero", "argwhere", "count_nonzero", "extract", "compress"):
     HANDLED_FUNCTIONS[_n] = globals()[_n]
 
 

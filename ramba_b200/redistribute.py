@@ -47,8 +47,10 @@ def run_local_offsets(size, m, local_strides, origin):
 
 def intersect_runs(a_start, a_len, b_start, b_len):
     """All non-empty intersections of two sorted families of equal-length, disjoint runs:
-    (index into a, index into b, linear start, length), ordered by linear start."""
-    if len(a_start) == 0 or len(b_start) == 0 or a_len == 0 or b_len == 0:
+    (index into a, index into b, linear start, length), ordered by linear start.  a_len may also be one length per run
+    of a (runs of a sorted and disjoint)."""
+    a_len = np.broadcast_to(np.asarray(a_len, dtype=np.int64), np.shape(a_start))
+    if len(a_start) == 0 or len(b_start) == 0 or not a_len.any() or b_len == 0:
         z = np.zeros(0, dtype=np.int64)
         return z, z, z, z
     lo = np.searchsorted(b_start + b_len, a_start, side="right")
@@ -59,7 +61,7 @@ def intersect_runs(a_start, a_len, b_start, b_len):
     first = np.repeat(np.cumsum(cnt) - cnt, cnt)
     ib = np.repeat(lo, cnt) + (np.arange(tot, dtype=np.int64) - first)
     s = np.maximum(a_start[ia], b_start[ib])
-    e = np.minimum(a_start[ia] + a_len, b_start[ib] + b_len)
+    e = np.minimum(a_start[ia] + a_len[ia], b_start[ib] + b_len)
     keep = e > s
     return ia[keep], ib[keep], s[keep], (e - s)[keep]
 

@@ -155,6 +155,14 @@ class CudaBackend:
         cabi.arg_reduce(view, src_code, axis, op, o, g, out_idx, out_key, scratch.data_ptr() if nbytes else None, self.stream_handle())
         return scratch
 
+    def compact_count(self, cond, cond_code, run_len, counts):
+        """rb200_compact_count on the current stream."""
+        cabi.compact_count(cond, cond_code, run_len, counts, self.stream_handle())
+
+    def compact(self, cond, cond_code, run_len, counts, incl, run_base, form, values, origin, gstride, outs):
+        """rb200_compact on the current stream."""
+        cabi.compact(cond, cond_code, run_len, counts, incl, run_base, form, values, origin, gstride, outs, self.stream_handle())
+
     def init_process_group(self):
         dist.init_process_group("nccl", device_id=self.device)
 
@@ -484,6 +492,18 @@ class Runtime:
         scratch = self.be().arg_reduce(view, src_code, axis, op, origin, gstride, out_idx, out_key)
         self.launches += 1
         return scratch
+
+    def compact_count(self, cond, cond_code, run_len, counts):
+        """Selected elements per chunk of one local condition view cut into runs of run_len C-order positions
+        (rb200_compact_count); counts: device address of n_runs * chunks-per-run int64."""
+        self.be().compact_count(cond, cond_code, run_len, counts)
+        self.launches += 1
+
+    def compact(self, cond, cond_code, run_len, counts, incl, run_base, form, values, origin, gstride, outs):
+        """The payload (cabi.COMPACT_VALUES / FLAT / COORDS) of every selected element of one local condition view, in C
+        order from run_base[r] + incl[q] - counts[q] for chunk q of run r (rb200_compact); outs: device addresses."""
+        self.be().compact(cond, cond_code, run_len, counts, incl, run_base, form, values, origin, gstride, outs)
+        self.launches += 1
 
     def gather(self, view, lin, n, out, bad):
         """out[i] = view[lin[i]] for n entries (rb200_gather; view: a cabi.IndexView); bad counts the out-of-range ones."""
