@@ -28,7 +28,10 @@ constexpr int kScanV = 8;
 constexpr int kScanTile = kScanV * kThreads;
 
 template <class A> __device__ __forceinline__ A scan_identity(int op);
-template <> __device__ __forceinline__ double scan_identity<double>(int op) { return CT<double>::get(red_identity_bits(op, RB200_T_F64)); }
+// -0.0 for a float sum: -0.0 + x is x for every x, so a run of -0.0 scans to -0.0 (NumPy's cumsum), where +0.0 would not
+template <> __device__ __forceinline__ double scan_identity<double>(int op) {
+  return op == RB200_RED_ADD ? -0.0 : CT<double>::get(red_identity_bits(op, RB200_T_F64));
+}
 template <> __device__ __forceinline__ long long scan_identity<long long>(int op) { return (long long)red_identity_bits(op, RB200_T_I64); }
 
 template <class A> __device__ __forceinline__ A shfl_up_a(A v, int d);

@@ -372,10 +372,10 @@ __device__ __forceinline__ void sterm_reduce(const StreamParams& P, const STermC
       for (int k = 0; k < TV; ++k) ip_mul(cacc[k], acc[k]);
     } else if (rop == RB200_RED_MIN) {
 #pragma unroll
-      for (int k = 0; k < TV; ++k) cacc[k] = acc[k] < cacc[k] ? acc[k] : cacc[k];
+      for (int k = 0; k < TV; ++k) cacc[k] = red_combine<double>(RB200_RED_MIN, cacc[k], acc[k]);
     } else {
 #pragma unroll
-      for (int k = 0; k < TV; ++k) cacc[k] = acc[k] > cacc[k] ? acc[k] : cacc[k];
+      for (int k = 0; k < TV; ++k) cacc[k] = red_combine<double>(RB200_RED_MAX, cacc[k], acc[k]);
     }
     return;
   }

@@ -406,13 +406,14 @@ __device__ __forceinline__ long long ipowi(long long a, long long b) {
   return r;
 }
 
-// reduction combine in the accumulator class (raw bits)
+// reduction combine in the accumulator class (raw bits).  MIN / MAX take a NaN from either side, so a NaN anywhere
+// reaches the result wherever it sits in the tree (NumPy's min / max); the elementwise min / max binops do not.
 template <class T> __device__ __forceinline__ T red_combine(int op, T a, T b) {
   switch (op) {
     case RB200_RED_ADD: return a + b;
     case RB200_RED_MUL: return a * b;
-    case RB200_RED_MIN: return (b < a) ? b : a;
-    default: return (b > a) ? b : a;
+    case RB200_RED_MIN: return (b < a || b != b) ? b : a;
+    default: return (b > a || b != b) ? b : a;
   }
 }
 __device__ __forceinline__ u64 red_combine_bits(int op, int ctype, u64 a, u64 b) {

@@ -22,7 +22,7 @@ import torch
 from . import _cabi as cabi
 from . import common
 from . import shardview
-from .program import E, REDUCTIONS, Lowering, ProgramError, rb_dtype
+from .program import REDUCTIONS, Lowering, ProgramError, fold_expr, rb_dtype
 from .runtime import RT, _VERIFY_PLAN_CACHE, fill_template, torch_dtype
 
 
@@ -46,7 +46,7 @@ def _combine_program(red_code, acc_code, combine):
     key = (red_code, acc_code, combine)
     if key not in _combine_programs:
         lw = Lowering([red_code, acc_code])
-        tv = lw.build(E(combine, lw.read_view(0), lw.read_view(1)), None)
+        tv = lw.build(fold_expr(combine, lw.read_view(0), lw.read_view(1)), None)
         lw.store(0, tv)
         _combine_programs[key] = lw.finish()
     return _combine_programs[key]

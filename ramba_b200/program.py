@@ -16,6 +16,8 @@ The reference's fuser accumulates *Python source lines* (`tmp_k = f(tmp_i, tmp_j
 The output (`Program`) is position independent: the same program is bound to every iteration
 range of a flush (ramba/ramba.py:3758-3780 calls the same compiled function per range).
 """
+import functools
+import operator
 import struct
 
 import numpy as np
@@ -73,13 +75,23 @@ class Reduction:
 
 
 REDUCTIONS = {
-    "sum": Reduction(cabi.RED_ADD, "add", "SUM", lambda dt: 0, lambda s: s.sum(0)),
+    # (the fold adds the rows in order from the first: torch's sum starts from +0.0 and would turn a -0.0 carry into +0.0)
+    "sum": Reduction(cabi.RED_ADD, "add", "SUM", lambda dt: 0, lambda s: functools.reduce(operator.add, s.unbind(0))),
     "prod": Reduction(cabi.RED_MUL, "mul", "PRODUCT", lambda dt: 1, lambda s: s.prod(0)),
     "min": Reduction(cabi.RED_MIN, "min", "MIN", lambda dt: getminmax(dt)[1], lambda s: s.min(0).values),
     "max": Reduction(cabi.RED_MAX, "max", "MAX", lambda dt: getminmax(dt)[0], lambda s: s.max(0).values),
     "all": Reduction(cabi.RED_MUL, "mul", "MIN", lambda dt: 1, lambda s: s.min(0).values, truth=True),
     "any": Reduction(cabi.RED_ADD, "add", "MAX", lambda dt: 0, lambda s: s.max(0).values, truth=True),
 }
+
+
+def fold_expr(combine, a, b):
+    """E folding partial b into partial a with a reduction's combine operator.  For min / max a NaN on either side
+    wins (NumPy's reductions); the min / max binop alone is builtins.min / max, which keeps a NaN only in a."""
+    e = E(combine, a, b)
+    if combine in ("min", "max"):
+        e = E("where", E("ne", b, b), b, e)
+    return e
 
 
 def red_identity(op, dtype):

@@ -32,8 +32,8 @@ from . import blocks
 from . import common
 from . import shardview
 from .common import dprint, timer, add_time
-from .flush import _combine_program, _contig_strides, _pack_program, _plan_cache, run_deferred_ops
-from .program import E, REDUCTIONS, Iota, Lowering, ProgramError, ProgramLimit, dtype_class, getminmax, rb_dtype, red_identity
+from .flush import _contig_strides, _pack_program, _plan_cache, run_deferred_ops
+from .program import E, REDUCTIONS, Iota, Lowering, ProgramError, ProgramLimit, dtype_class, fold_expr, getminmax, rb_dtype, red_identity
 from .runtime import RT, torch_dtype
 
 int64 = np.int64
@@ -1459,6 +1459,25 @@ def _local_partial_tensor(red_arr, n, op):
     return sh.interior().reshape(-1)[:n].to(acc_dt)
 
 
+_KEY_FLIP = 0x7FFFFFFFFFFFFFFF
+
+
+def _all_reduce_partials(t, op):
+    """t = op over every rank's partials, in place.  Float min / max reduce order-preserving int64 keys of the float64
+    bits with NaN beyond every number, so a NaN on any rank wins (NumPy) whatever the backend's float MIN / MAX do with
+    NaN; one collective, as for sum."""
+    if op not in ("min", "max") or not t.is_floating_point():
+        RT.all_reduce(t, op)
+        return
+    nan_key = torch.iinfo(torch.int64).min if op == "min" else torch.iinfo(torch.int64).max
+    bits = t.view(torch.int64)
+    key = torch.where(bits < 0, bits ^ _KEY_FLIP, bits)
+    key = torch.where(torch.isnan(t), nan_key, key)
+    RT.all_reduce(key, op)
+    val = torch.where(key < 0, key ^ _KEY_FLIP, key).view(torch.float64)
+    t.copy_(torch.where(key == nan_key, float("nan"), val))
+
+
 def _reduction2b(red_arr, op, dtype, asarray):
     """Stage 2 of a global reduction.  The reference gathers one partial per worker to the driver and reduces them
     there (ramba/ramba.py:5852-5863); under SPMD every rank needs the result, so the partials (one element per rank,
@@ -1473,7 +1492,7 @@ def _reduction2b(red_arr, op, dtype, asarray):
     if common.num_workers > 1:
         DAG.instantiate(red_arr)
         t = _local_partial_tensor(red_arr, 1, op)
-        RT.all_reduce(t, op)
+        _all_reduce_partials(t, op)
         val = t.cpu().numpy()[0]
         if REDUCTIONS[op].truth:
             val = np.bool_(val != 0)
@@ -1518,7 +1537,7 @@ def _reduction2(red_arr, op, dtype, axis, keepdims):
         DAG.instantiate(red_arr)
         w = common.worker_num
         t = _local_partial_tensor(red_arr, kept_elems, op)
-        RT.all_reduce(t, op)
+        _all_reduce_partials(t, op)
         out_shape = tuple(1 if d in axis else red_arr.shape[d] for d in range(nd))
         arr = ndarray(out_shape, dtype=red_arr.dtype, flex_dist=False)
         sh = blocks.block(arr)
@@ -1540,7 +1559,7 @@ def _reduction2(red_arr, op, dtype, axis, keepdims):
             else:
                 sl.append(slice(None))
         piece = red_arr[tuple(sl)]
-        expr = piece if expr is None else E(combine, expr, piece)
+        expr = piece if expr is None else fold_expr(combine, expr, piece)
     DAG.assign(arr, expr)
     return arr[sl1]
 
@@ -2793,7 +2812,7 @@ def _scan_native(a, axis, kind, dtype):
     totals = torch.empty(max(1, ncols), dtype=acc_dt, device=RT.device) if split_axis else None
     if totals is not None:
         totals.fill_(red.identity(out_dtype))
-    scratch = carry = None
+    scratch = carry = rescan = None
     if not mine_empty:
         scratch = RT.cumulative(sh_src.ptr(0), sh_res.ptr(0), code, n_outer, length, n_inner, red.code, None, totals.data_ptr() if totals is not None else None)
     if split_axis and W > 1:
@@ -2804,11 +2823,10 @@ def _scan_native(a, axis, kind, dtype):
             if before:
                 stack = allt.view(W, ncols)[before]
                 carry = red.fold(stack).contiguous()
-                acc_code = cabi.F64 if acc_dt == torch.float64 else cabi.I64
-                # res[o, l, i] = carry[o, i] (op) res[o, l, i] for every l: one fused op with the carry broadcast along the axis
-                RT.launch(_combine_program(code, acc_code, red.combine), [n_outer, length, n_inner], [0, 0, 0],
-                          [(sh_res.ptr(0), [length * n_inner, n_inner, 1], code, sh_res.bounds), (carry.data_ptr(), [n_inner, 0, 1], acc_code)])
-    RT.hold(scratch, carry)  # (read only by the launches above)
+                # scan the block again seeded with the carry, so that the carry joins the float64 accumulator and every
+                # element is rounded once, as at one rank (folding the carry into the stored result would round twice)
+                rescan = RT.cumulative(sh_src.ptr(0), sh_res.ptr(0), code, n_outer, length, n_inner, red.code, carry.data_ptr(), None)
+    RT.hold(scratch, carry, rescan)  # (read only by the launches above)
     return res
 
 
