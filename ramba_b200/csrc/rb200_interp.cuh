@@ -90,8 +90,8 @@ template <class R> __device__ __forceinline__ void store_one(char* base, int dty
   switch (dtype) {
     case RB200_F64: reinterpret_cast<double*>(base)[off] = (double)x; break;
     case RB200_F32: reinterpret_cast<float*>(base)[off] = (float)x; break;
-    case RB200_I64: reinterpret_cast<long long*>(base)[off] = (long long)x; break;
-    case RB200_I32: reinterpret_cast<int*>(base)[off] = (int)x; break;
+    case RB200_I64: reinterpret_cast<long long*>(base)[off] = to_i64<R>(x); break;
+    case RB200_I32: reinterpret_cast<int*>(base)[off] = to_storage<int>(x); break;
     default: store_narrow_one<R>(base, dtype, off, x);
   }
 }
@@ -640,8 +640,9 @@ template <int V, class C> __device__ __forceinline__ void exec_int(C& cx, const 
                : op == RB200_OP_BAND ? (x & y)
                : op == RB200_OP_BOR  ? (x | y)
                : op == RB200_OP_BXOR ? (x ^ y)
-               : op == RB200_OP_SHL  ? (long long)((u64)x << (y & 63))
-                                     : (x >> (y & 63));
+               // counts outside [0, 63] shift every bit out, as NumPy's: 0, or -1 for a right shift of a negative x
+               : op == RB200_OP_SHL  ? ((u64)y < 64 ? (long long)((u64)x << y) : 0)
+                                     : ((u64)y < 64 ? (x >> y) : (x < 0 ? -1 : 0));
       }
       break;
     case RB200_OP_FLOORDIV:
@@ -728,20 +729,17 @@ template <int V, class C> __device__ __forceinline__ void exec_int(C& cx, const 
   cx.template finish<long long>(I, r);
 }
 
-// value a store + reload through storage dtype `dt` would give (narrowing round / wrap)
-template <class T> __device__ __forceinline__ T through_storage(T x, int dt) {
+// value a store + reload through integer storage dtype `dt` would give (wrap), as an int64
+template <class T> __device__ __forceinline__ long long through_int(T x, int dt) {
   switch (dt) {
-    case RB200_F64: return (T)(double)x;
-    case RB200_F32: return (T)(float)x;
-    case RB200_I64: return (T)(long long)x;
-    case RB200_I32: return (T)(int)x;
-    case RB200_BOOL: return (T)(x != T(0) ? 1 : 0);
-    case RB200_U8: return (T)(unsigned char)(long long)x;
-    case RB200_I8: return (T)(signed char)(long long)x;
-    case RB200_I16: return (T)(short)(long long)x;
-    case RB200_U16: return (T)(unsigned short)(long long)x;
-    case RB200_U32: return (T)(unsigned int)(long long)x;
-    default: return x;
+    case RB200_I32: return to_storage<int>(x);
+    case RB200_BOOL: return x != T(0) ? 1 : 0;
+    case RB200_U8: return to_storage<unsigned char>(x);
+    case RB200_I8: return to_storage<signed char>(x);
+    case RB200_I16: return to_storage<short>(x);
+    case RB200_U16: return to_storage<unsigned short>(x);
+    case RB200_U32: return to_storage<unsigned int>(x);
+    default: return to_i64<T>(x);
   }
 }
 
@@ -749,9 +747,17 @@ template <class S, int V, class C> __device__ __forceinline__ void exec_cvt_from
   S a[V];
   cx.template fetch<S>(I.a_kind(), I.a_idx(), a);
   const int through = (int)(I.imm() >> 8);
-  if (through != 0) {
+  if (through - 1 == RB200_F64 || through - 1 == RB200_F32) {
 #pragma unroll
-    for (int k = 0; k < V; ++k) a[k] = through_storage<S>(a[k], through - 1);
+    for (int k = 0; k < V; ++k) a[k] = through - 1 == RB200_F64 ? (S)(double)a[k] : (S)(float)a[k];
+  } else if (through != 0) {
+    // an integer storage dtype: the reloaded value is the wrapped integer itself, which the class of `a` (float32 above
+    // 2^24) may not hold - go straight to the int64 class
+    long long r[V];
+#pragma unroll
+    for (int k = 0; k < V; ++k) r[k] = through_int<S>(a[k], through - 1);
+    cx.template finish<long long>(I, r);
+    return;
   }
   switch (I.ctype()) {
     case RB200_T_F64: {
@@ -769,7 +775,7 @@ template <class S, int V, class C> __device__ __forceinline__ void exec_cvt_from
     default: {
       long long r[V];
 #pragma unroll
-      for (int k = 0; k < V; ++k) r[k] = (long long)a[k];
+      for (int k = 0; k < V; ++k) r[k] = to_i64<S>(a[k]);
       cx.template finish<long long>(I, r);
     }
   }
@@ -882,7 +888,7 @@ template <class TS, class TD, int AK, int V, class C> __device__ __forceinline__
   TD r[V];
   fetch_s<TS, AK, V>(cx, I.a_idx(), a);
 #pragma unroll
-  for (int k = 0; k < V; ++k) r[k] = (TD)a[k];
+  for (int k = 0; k < V; ++k) r[k] = to_storage<TD>(a[k]);  // float -> int64 by to_i64, not the saturating C cast
   cx.template finish<TD>(I, r);
 }
 

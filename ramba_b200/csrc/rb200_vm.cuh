@@ -15,6 +15,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 #include "../../include/ramba_b200.h"
 
 namespace rb200 {
@@ -155,8 +156,22 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // ---------------------------------------------------------------------------------------------
+// Float -> integer, one rule on every path (CVT, converting stores, store + reload through a storage dtype): NaN, +-inf
+// and |x| >= 2^63 give INT64_MIN, anything else truncates toward zero, and a narrower integer dtype keeps the low bits
+// of that int64.  This is what NumPy's astype(int64) gives on x86-64; a bare C cast would be PTX cvt.rzi, which clamps
+// to the destination (+inf -> INT64_MAX, NaN -> 0, 3e9 -> int32 2147483647).
+template <class T> __device__ __forceinline__ long long to_i64(T x) {
+  if constexpr (std::is_floating_point<T>::value) return fabs(x) < T(9223372036854775808.0) ? (long long)x : (long long)0x8000000000000000ull;
+  else return (long long)x;
+}
+// x as storage type S: integers through to_i64, floats by the C cast (int->float rn, f64->f32 rn)
+template <class S, class T> __device__ __forceinline__ S to_storage(T x) {
+  if constexpr (std::is_integral<S>::value) return (S)to_i64<T>(x);
+  else return (S)x;
+}
+
+// ---------------------------------------------------------------------------------------------
 // element loads / stores through explicit global-space instructions.
-// C cast semantics == Numba/LLVM casts (float->int truncates, int->float rn, f64->f32 rn).
 template <class S> __device__ __forceinline__ S ldg(const S* p) { return *p; }
 template <> __device__ __forceinline__ double ldg<double>(const double* p) {
   double v;
@@ -234,17 +249,17 @@ __device__ __forceinline__ void store_direct(char* base, const long long (&off)[
   S* p = reinterpret_cast<S*>(base);
 #pragma unroll
   for (int k = 0; k < V; ++k)
-    if ((mask >> k) & 1u) stg<S>(p + off[k], (S)val[k]);
+    if ((mask >> k) & 1u) stg<S>(p + off[k], to_storage<S>(val[k]));
 }
 
 template <class T> __device__ __noinline__ void store_narrow_one(char* base, int dtype, long long off, T x) {
   switch (dtype) {
     case RB200_BOOL: reinterpret_cast<unsigned char*>(base)[off] = (x != T(0)) ? 1 : 0; break;
-    case RB200_U8: reinterpret_cast<unsigned char*>(base)[off] = (unsigned char)(long long)x; break;
-    case RB200_I8: reinterpret_cast<signed char*>(base)[off] = (signed char)(long long)x; break;
-    case RB200_I16: reinterpret_cast<short*>(base)[off] = (short)(long long)x; break;
-    case RB200_U16: reinterpret_cast<unsigned short*>(base)[off] = (unsigned short)(long long)x; break;
-    case RB200_U32: reinterpret_cast<unsigned int*>(base)[off] = (unsigned int)(long long)x; break;
+    case RB200_U8: reinterpret_cast<unsigned char*>(base)[off] = to_storage<unsigned char>(x); break;
+    case RB200_I8: reinterpret_cast<signed char*>(base)[off] = to_storage<signed char>(x); break;
+    case RB200_I16: reinterpret_cast<short*>(base)[off] = to_storage<short>(x); break;
+    case RB200_U16: reinterpret_cast<unsigned short*>(base)[off] = to_storage<unsigned short>(x); break;
+    case RB200_U32: reinterpret_cast<unsigned int*>(base)[off] = to_storage<unsigned int>(x); break;
     default: break;
   }
 }
@@ -346,15 +361,17 @@ template <int V> __device__ __forceinline__ void sincos_v(const float (&x)[V], f
 // ---------------------------------------------------------------------------------------------
 // scalar op semantics
 
-// Python floor division / modulo (what Numba emits for `//` and `%`)
+// Python floor division / modulo (what Numba emits for `//` and `%`).  A zero divisor gives 0 (no trap), and b = -1
+// never reaches the hardware divide, whose INT64_MIN / -1 is undefined: the quotient wraps to INT64_MIN as NumPy's does.
 __device__ __forceinline__ long long py_floordiv(long long a, long long b) {
   if (b == 0) return 0;
+  if (b == -1) return (long long)(0ull - (u64)a);
   long long q = a / b;
   if ((a % b != 0) && ((a < 0) != (b < 0))) --q;
   return q;
 }
 __device__ __forceinline__ long long py_mod(long long a, long long b) {
-  if (b == 0) return 0;
+  if (b == 0 || b == -1) return 0;
   long long r = a % b;
   if (r != 0 && ((r < 0) != (b < 0))) r += b;
   return r;
@@ -369,7 +386,9 @@ template <class F> __device__ __forceinline__ F py_fmod(F a, F b) {
   return r;
 }
 template <class F> __device__ __forceinline__ F py_ffloordiv(F a, F b) {
-  // CPython float_floor_div / Numba real_floordiv
+  // CPython float_floor_div / Numba real_floordiv; a zero divisor gives a / b (+-inf, NaN for 0 / 0) as in Numba and
+  // NumPy, where fmod(a, 0) = NaN would otherwise fall through to the result
+  if (b == F(0)) return a / b;
   F mod = fmod(a, b);
   F div = (a - mod) / b;
   if (mod != F(0) && ((b < F(0)) != (mod < F(0)))) div -= F(1);
