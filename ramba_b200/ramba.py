@@ -1146,26 +1146,32 @@ class ndarray:
                 axis = None
         red = REDUCTIONS[op]
         init = red.identity(dtype)
+        src = self
         if red.truth:
             init = bool(init)  # (the partial array of all / any starts as a truth value)
+            # reduce each element's truth value: a product or sum of 0/1 cannot wrap, underflow, reach NaN or cancel
+            src = E("ne", self, 0)
+        elif dtype_class(rb_dtype(dtype)) != dtype_class(rb_dtype(self.dtype)):
+            src = E("astype", self, imm=rb_dtype(dtype))  # sum / prod(dtype=D): each element is converted to D first
         if self.maskarray is not None:
             axis = None
         if axis is None or (axis == [0] and self.ndim == 1):
             dsz, dist, bdist = shardview.reduce_all_axes(self.shape, self.distribution)
             red_arr = full(dsz, init, dtype=dtype, distribution=dist, no_defer=True)
             red_bcast = ndarray(self.shape, base=red_arr, distribution=bdist, local_border=0, readonly=False)
-            DAG.reduce(op, self if self.maskarray is None else E("where", self.maskarray, self, red_identity(op, dtype)),
+            DAG.reduce(op, src if self.maskarray is None else E("where", self.maskarray, src, red_identity(op, dtype)),
                        red_bcast, elide=elide)
             return _reduction2b(red_arr, op, dtype, asarray)
         dsz, dist, bdist = shardview.reduce_axes(self.shape, self.distribution, axis)
         red_arr = full(dsz, init, dtype=dtype, distribution=dist, no_defer=True)
         red_bcast = ndarray(self.shape, base=red_arr, distribution=bdist, local_border=0, readonly=False)
-        DAG.reduce(op, self, red_bcast, axis, elide)
+        DAG.reduce(op, src, red_bcast, axis, elide)
         return _reduction2(red_arr, op, dtype, axis, keepdims is True)
 
     def mean(self, axis=None, dtype=None, **kwargs):
         n = self.size if axis is None else int(np.prod([self.shape[a] for a in ([axis] if isinstance(axis, numbers.Number) else axis)]))
-        s = self.sum(axis=axis, **kwargs)
+        # integer and bool data: NumPy's float64 sum of float64(x) (an integer sum would wrap, a bool sum is an `or`)
+        s = self.sum(axis=axis, dtype=np.float64 if self.dtype.kind in "iub" else None, **kwargs)
         if dtype is None:
             dtype = np.float64 if self.dtype.kind in "iub" else self.dtype
         if isinstance(s, ndarray):
@@ -1391,7 +1397,8 @@ class ndarray:
         """Mean of the elements that are not NaN (whole array, like the reference: ramba/ramba.py:6766-6772)."""
         assert axis is None, "nanmean over an axis is not implemented (nor by the reference, ramba/ramba.py:6760-6763)"
         ok = isnan(self).logical_not()  # noqa: F821
-        return self[ok].sum() / ok.astype(np.int64).sum()  # (a bool sum stays bool, like in the reference)
+        s = self[ok].sum(dtype=np.float64 if self.dtype.kind in "iub" else None)  # (as in mean)
+        return s / ok.astype(np.int64).sum()  # (a bool sum stays bool, like in the reference)
 
     def rollaxis(self, axis, start=0):
         """NumPy's rollaxis (ramba/ramba.py:5643-5654)."""
