@@ -420,6 +420,60 @@ int rb200_compact(const rb200_index_view* cond, int32_t cond_dtype, int64_t run_
  * the next call on this thread.                                                                                       */
 const char* rb200_describe_compact_plan(const rb200_index_view* cond, int64_t run_len);
 
+/* ---- binning (histogram, bincount, digitize, searchsorted) -----------------------------------------------------------
+ * rb200_histogram bins every element of the source view into B bins described by an rb200_bin_table:
+ *   RB200_BINS_UNIFORM: NumPy's equal-bins path (numpy/lib/_histograms_impl.py::histogram) on each element x: it is kept
+ *     when first <= x (compared in lo_dtype) and x <= last (in hi_dtype); x is converted to edge_dtype (xe), then
+ *     i = trunc(((xe - first) / denom) * B), the subtraction rounded in sub_dtype and the division and product in
+ *     div_dtype, with no contraction; i == B becomes B - 1; then i -= 1 when xe < edges[i], and i += 1 when
+ *     i != B - 1 and xe >= edges[i + 1].  An index that leaves [0, B) is counted in *bad.
+ *   RB200_BINS_EDGES: x (converted to edge_dtype, the comparison dtype) lands in bin i when edges[i] <= x < edges[i + 1],
+ *     the last bin closed, in NumPy's sort order (NaN after every number); other values are dropped.
+ *   RB200_BINS_INTEGER: the bin is x itself (an integer source); an element outside [0, B) is counted in *bad.
+ * Without weights, out receives B int64 counts; with weights (a view of the source's shape, F64 / F32 / I64 / I32) it
+ * receives B float64 sums of the weights converted to float64.  src_dtype: F64, F32, I64 or I32 (INTEGER: I64 or I32).
+ * *bad (device, may be NULL when the form cannot produce one) is added to, never reset.
+ * Forms (rb200_describe_hist_plan): CTA c covers the C-order positions [c * chunk, (c + 1) * chunk), chunk a function of
+ * the view's size only.  `shared`: per-CTA bins in shared memory; `global`: counts too many for shared memory, added
+ * with int64 atomics; `slab`: weights too many for shared memory, one pass of the shared form per slab of bins.
+ * Fold order of a weighted bin (a function of the view's shape, B, the form and the source's element size only): inside
+ * a CTA each warp keeps its own row; the warp takes steps of 32 lanes * E elements (E = 16 / element bytes) in
+ * position order, and for each element slot of a step the weights of the lanes in one bin are added in ascending lane
+ * order and that sum is added to the row; the CTA's rows are added in warp order starting from +0.0, and the CTA sums
+ * in CTA order starting from +0.0.  No float atomics.  An empty bin, or one holding only -0.0, is +0.0.
+ * scratch: rb200_histogram_scratch_bytes() bytes (may be NULL when that is 0).                                        */
+enum rb200_bins_form { RB200_BINS_UNIFORM = 0, RB200_BINS_EDGES = 1, RB200_BINS_INTEGER = 2 };
+enum rb200_search_side { RB200_SEARCH_LEFT = 0, RB200_SEARCH_RIGHT = 1 };
+
+typedef struct rb200_bin_table {
+  int32_t form;         /* rb200_bins_form                                                                        */
+  int32_t edge_dtype;   /* UNIFORM: F64 or F32; EDGES: F64, F32 or I64                                           */
+  int64_t n_bins;       /* B, 1 .. 2^31 - 1                                                                       */
+  const void* edges;    /* device, B + 1 entries of edge_dtype, non-decreasing (UNIFORM, EDGES)                   */
+  int32_t lo_dtype;     /* UNIFORM: F64, F32 or I64                                                               */
+  int32_t hi_dtype;
+  int32_t sub_dtype;    /* UNIFORM: F64 or F32, not narrower than edge_dtype                                      */
+  int32_t div_dtype;    /* UNIFORM: F64 or F32, not narrower than sub_dtype                                       */
+  double lo, hi;        /* UNIFORM: first and last for F64 / F32 comparisons (F32: a float32 value)               */
+  int64_t lo_i, hi_i;   /* UNIFORM: first and last for I64 comparisons                                            */
+  double first;         /* UNIFORM: first in sub_dtype                                                            */
+  double denom;         /* UNIFORM: NumPy's last - first in div_dtype                                             */
+} rb200_bin_table;
+
+int rb200_histogram(const rb200_index_view* src, int32_t src_dtype, const rb200_index_view* weights, int32_t weights_dtype,
+                    const rb200_bin_table* table, void* out, uint64_t* bad, void* scratch, void* stream);
+int64_t rb200_histogram_scratch_bytes(const rb200_index_view* src, int32_t weighted, const rb200_bin_table* table);
+/* One text line: form, chunk, CTAs, warps, shared bytes, passes, where the edge table is read and scratch.  Needs no
+ * device.  NULL on a malformed argument (reason in rb200_last_error); valid until the next call on this thread.       */
+const char* rb200_describe_hist_plan(const rb200_index_view* src, int32_t weighted, const rb200_bin_table* table);
+
+/* out[p] (device, contiguous, one int64 per element in the view's C order) = the number of entries of the sorted table
+ * (device, n_sorted entries of sorted_dtype F64, F32 or I64, the comparison dtype) that are below x (side LEFT) or not
+ * above x (side RIGHT), x converted to sorted_dtype, in NumPy's order (NaN after every number): NumPy's searchsorted.
+ * src_dtype: F64, F32, I64 or I32.                                                                                    */
+int rb200_bin_search(const rb200_index_view* src, int32_t src_dtype, const void* sorted, int64_t n_sorted, int32_t sorted_dtype, int32_t side,
+                     int64_t* out, void* stream);
+
 /* Which kernel rb200_run_deferred_ops would run `op` on and how (staged views, halos, TMA or cp.async loader, ring depth,
  * lean instructions, CTAs), as one text line in out[0..cap).  Needs no device and touches no pointer: the counterpart
  * of RAMBA_SHOW_CODE printing the generated kernel (ramba/ramba.py:8266-8284).                                       */

@@ -45,6 +45,9 @@ ARG_ALL_AXES = -1
 # stream-compaction payload forms (rb200_compact) and its chunk size
 COMPACT_VALUES, COMPACT_FLAT, COMPACT_COORDS = range(3)
 COMPACT_CHUNK = 4096
+# binning: bin-table forms (rb200_histogram) and search sides (rb200_bin_search)
+BINS_UNIFORM, BINS_EDGES, BINS_INTEGER = range(3)
+SEARCH_LEFT, SEARCH_RIGHT = range(2)
 
 
 class Insn(C.Structure):
@@ -107,6 +110,18 @@ class IndexView(C.Structure):
     ]
 
 
+class BinTable(C.Structure):
+    _fields_ = [
+        ("form", C.c_int32), ("edge_dtype", C.c_int32),
+        ("n_bins", C.c_int64),
+        ("edges", C.c_void_p),
+        ("lo_dtype", C.c_int32), ("hi_dtype", C.c_int32), ("sub_dtype", C.c_int32), ("div_dtype", C.c_int32),
+        ("lo", C.c_double), ("hi", C.c_double),
+        ("lo_i", C.c_int64), ("hi_i", C.c_int64),
+        ("first", C.c_double), ("denom", C.c_double),
+    ]
+
+
 class RouteTable(C.Structure):
     _fields_ = [
         ("ndim", C.c_int32), ("n_ranks", C.c_int32),
@@ -157,6 +172,10 @@ EXPORTS = [
     "rb200_compact_count",
     "rb200_compact",
     "rb200_describe_compact_plan",
+    "rb200_histogram",
+    "rb200_histogram_scratch_bytes",
+    "rb200_describe_hist_plan",
+    "rb200_bin_search",
 ]
 
 _LIB = None
@@ -236,6 +255,15 @@ def load():
     lib.rb200_compact.restype = C.c_int
     lib.rb200_describe_compact_plan.argtypes = [C.POINTER(IndexView), C.c_int64]
     lib.rb200_describe_compact_plan.restype = C.c_char_p
+    lib.rb200_histogram.argtypes = [C.POINTER(IndexView), C.c_int32, C.POINTER(IndexView), C.c_int32, C.POINTER(BinTable), C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.rb200_histogram.restype = C.c_int
+    lib.rb200_histogram_scratch_bytes.argtypes = [C.POINTER(IndexView), C.c_int32, C.POINTER(BinTable)]
+    lib.rb200_histogram_scratch_bytes.restype = C.c_int64
+    lib.rb200_describe_hist_plan.argtypes = [C.POINTER(IndexView), C.c_int32, C.POINTER(BinTable)]
+    lib.rb200_describe_hist_plan.restype = C.c_char_p
+    lib.rb200_bin_search.argtypes = [C.POINTER(IndexView), C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.rb200_bin_search.restype = C.c_int
     if lib.rb200_abi_version() != ABI_VERSION:
         raise CabiError("libramba_b200.so ABI %d != binding ABI %d: rebuild" % (lib.rb200_abi_version(), ABI_VERSION))
     _LIB = lib
@@ -434,3 +462,29 @@ def describe_compact_plan(cond, run_len):
     if s is None:
         check(1)
     return s.decode()
+
+
+def histogram(src, src_dtype, weights, weights_dtype, table, out, bad, scratch, stream=None):
+    """rb200_histogram: this view's B int64 counts (weights None) or float64 weight sums into out (device)."""
+    check(load().rb200_histogram(C.byref(src), src_dtype, C.byref(weights) if weights is not None else None, weights_dtype,
+                                 C.byref(table), _p(out), _p(bad), _p(scratch), _p(stream)))
+
+
+def histogram_scratch_bytes(src, weighted, table):
+    n = load().rb200_histogram_scratch_bytes(C.byref(src), int(bool(weighted)), C.byref(table))
+    if n < 0:
+        check(1)
+    return n
+
+
+def describe_hist_plan(src, weighted, table):
+    """One text line: the form, chunk, CTAs, shared bytes and passes the library would bin this view with (no device)."""
+    s = load().rb200_describe_hist_plan(C.byref(src), int(bool(weighted)), C.byref(table))
+    if s is None:
+        check(1)
+    return s.decode()
+
+
+def bin_search(src, src_dtype, sorted_ptr, n_sorted, sorted_dtype, side, out, stream=None):
+    """rb200_bin_search: out[p] (device int64, the view's C order) = NumPy's searchsorted of every element."""
+    check(load().rb200_bin_search(C.byref(src), src_dtype, _p(sorted_ptr), n_sorted, sorted_dtype, side, _p(out), _p(stream)))

@@ -11,6 +11,7 @@
 #include "rb200_plan.h"
 #include "rb200_argred.h"
 #include "rb200_compact.h"
+#include "rb200_hist.h"
 #include "rb200_group.h"
 #include "rb200_index.h"
 #include "rb200_rng.h"
@@ -407,6 +408,71 @@ static bool compact_is_float(int dt) { return dt == RB200_F64 || dt == RB200_F32
 
 static thread_local std::string g_compact_plan_text;
 
+// ---- binning: argument checks (before any device query) and the plans
+static bool bins_src_dtype(int dt) { return dt == RB200_F64 || dt == RB200_F32 || dt == RB200_I64 || dt == RB200_I32; }
+static bool bins_float_dtype(int dt) { return dt == RB200_F64 || dt == RB200_F32; }
+static bool bins_cmp_dtype(int dt) { return dt == RB200_F64 || dt == RB200_F32 || dt == RB200_I64; }
+
+static int check_bin_table(const rb200_bin_table* T) {
+  if (!T) return fail("histogram: null bin table");
+  if (T->form != RB200_BINS_UNIFORM && T->form != RB200_BINS_EDGES && T->form != RB200_BINS_INTEGER) return fail("histogram: bad bin table form");
+  if (T->n_bins < 1 || T->n_bins > 0x7fffffffll) return fail("histogram: n_bins must be in 1 .. 2^31 - 1");
+  if (T->form == RB200_BINS_UNIFORM) {
+    if (!bins_float_dtype(T->edge_dtype)) return fail("histogram: uniform edges must be float64 or float32");
+    if (!bins_cmp_dtype(T->lo_dtype) || !bins_cmp_dtype(T->hi_dtype)) return fail("histogram: bad bound dtype");
+    if (!bins_float_dtype(T->sub_dtype) || !bins_float_dtype(T->div_dtype)) return fail("histogram: bad arithmetic dtype");
+    if ((T->edge_dtype == RB200_F64 && T->sub_dtype != RB200_F64) || (T->sub_dtype == RB200_F64 && T->div_dtype != RB200_F64))
+      return fail("histogram: arithmetic dtype narrower than the edges");
+  } else if (T->form == RB200_BINS_EDGES && !bins_cmp_dtype(T->edge_dtype)) {
+    return fail("histogram: bad edge dtype");
+  }
+  if (T->form != RB200_BINS_INTEGER && !T->edges) return fail("histogram: null edges");
+  return 0;
+}
+
+static int check_hist_plan(const rb200_index_view* src, bool weighted, const rb200_bin_table* T, HistPlan* P) {
+  if (const int rc = check_index_view(src, "histogram")) return rc;
+  if (const int rc = check_bin_table(T)) return rc;
+  make_hist_plan(*src, weighted, *T, P);
+  return 0;
+}
+
+static int check_hist_dtypes(const rb200_index_view* src, int src_dtype, const rb200_index_view* weights, int weights_dtype, const rb200_bin_table* T) {
+  if (!bins_src_dtype(src_dtype)) return fail("histogram: source dtype must be float64/float32/int64/int32");
+  if (dtype_size(src_dtype) != src->elem_bytes) return fail("histogram: elem_bytes does not match the source dtype");
+  const bool fl = bins_float_dtype(src_dtype);
+  if (fl && T->form == RB200_BINS_INTEGER) return fail("histogram: integer bins need an integer source");
+  if (fl && T->form == RB200_BINS_EDGES && T->edge_dtype == RB200_I64) return fail("histogram: integer edges need an integer source");
+  if (fl && T->form == RB200_BINS_UNIFORM && (T->lo_dtype == RB200_I64 || T->hi_dtype == RB200_I64))
+    return fail("histogram: integer bounds need an integer source");
+  if (!weights) return 0;
+  if (const int rc = check_index_view(weights, "histogram weights")) return rc;
+  if (!bins_src_dtype(weights_dtype)) return fail("histogram: weights dtype must be float64/float32/int64/int32");
+  if (dtype_size(weights_dtype) != weights->elem_bytes) return fail("histogram: elem_bytes does not match the weights dtype");
+  if (weights->ndim != src->ndim) return fail("histogram: weights and source differ in shape");
+  for (int d = 0; d < src->ndim; ++d)
+    if (weights->shape[d] != src->shape[d]) return fail("histogram: weights and source differ in shape");
+  return 0;
+}
+
+static thread_local std::string g_hist_plan_text;
+
+static int check_search_args(const rb200_index_view* src, int src_dtype, const void* sorted, long long n_sorted, int sorted_dtype, int side,
+                             SearchPlan* P) {
+  if (const int rc = check_index_view(src, "bin_search")) return rc;
+  if (!bins_src_dtype(src_dtype)) return fail("bin_search: source dtype must be float64/float32/int64/int32");
+  if (dtype_size(src_dtype) != src->elem_bytes) return fail("bin_search: elem_bytes does not match the source dtype");
+  if (!bins_cmp_dtype(sorted_dtype)) return fail("bin_search: table dtype must be float64/float32/int64");
+  if (sorted_dtype == RB200_I64 && bins_float_dtype(src_dtype)) return fail("bin_search: an integer table needs an integer source");
+  if (n_sorted < 0) return fail("bin_search: negative table length");
+  if (n_sorted > 0 && !sorted) return fail("bin_search: null table");
+  if (side != RB200_SEARCH_LEFT && side != RB200_SEARCH_RIGHT) return fail("bin_search: bad side");
+  make_search_plan(*src, n_sorted, sorted_dtype, P);
+  P->src_dtype = src_dtype;
+  P->side = side;
+  return 0;
+}
+
 extern "C" {
 
 const char* rb200_last_error(void) { return g_last_error.c_str(); }
@@ -651,6 +717,56 @@ int rb200_compact(const rb200_index_view* cond, int32_t cond_dtype, int64_t run_
   const cudaError_t e = launch_compact(P, compact_is_float(cond_dtype), (const long long*)counts, (const long long*)incl, (const long long*)run_base, O,
                                        (cudaStream_t)stream_v);
   if (e != cudaSuccess) return fail_cuda("compact kernel launch", e);
+  g_launches.fetch_add(1);
+  return 0;
+}
+
+const char* rb200_describe_hist_plan(const rb200_index_view* src, int32_t weighted, const rb200_bin_table* table) {
+  HistPlan P;
+  if (check_hist_plan(src, weighted != 0, table, &P)) return nullptr;
+  char buf[320];
+  snprintf(buf, sizeof(buf),
+           "kernel=hist form=%s bins=%lld chunk=%lld ctas=%lld warps=%d shared_bytes=%lld passes=%lld slab=%lld table=%s load=%s scratch=%lld",
+           hist_form_name(P.form), P.B, P.chunk, P.ctas, 8, P.shared_bytes, P.passes, P.slab,
+           table->form == RB200_BINS_INTEGER ? "none" : P.table_shared ? "shared" : "global", P.vec ? "vector" : "strided", P.scratch_bytes);
+  g_hist_plan_text = buf;
+  return g_hist_plan_text.c_str();
+}
+
+int64_t rb200_histogram_scratch_bytes(const rb200_index_view* src, int32_t weighted, const rb200_bin_table* table) {
+  HistPlan P;
+  if (check_hist_plan(src, weighted != 0, table, &P)) return -1;
+  return P.scratch_bytes;
+}
+
+int rb200_histogram(const rb200_index_view* src, int32_t src_dtype, const rb200_index_view* weights, int32_t weights_dtype,
+                    const rb200_bin_table* table, void* out, uint64_t* bad, void* scratch, void* stream_v) {
+  HistPlan P;
+  if (const int rc = check_hist_plan(src, weights != nullptr, table, &P)) return rc;
+  if (const int rc = check_hist_dtypes(src, src_dtype, weights, weights_dtype, table)) return rc;
+  P.src_dtype = src_dtype;
+  P.w_dtype = weights_dtype;
+  if (!out) return fail("histogram: null out");
+  if (!bad && table->form != RB200_BINS_EDGES) return fail("histogram: null bad counter");
+  if (P.n > 0 && P.scratch_bytes > 0 && !scratch) return fail("histogram: null scratch");
+  int sms;
+  if (const int rc = need_device(&sms)) return rc;
+  const cudaError_t e = launch_histogram(P, *table, weights, out, (unsigned long long*)bad, scratch, (cudaStream_t)stream_v);
+  if (e != cudaSuccess) return fail_cuda("histogram kernel launch", e);
+  g_launches.fetch_add(1);
+  return 0;
+}
+
+int rb200_bin_search(const rb200_index_view* src, int32_t src_dtype, const void* sorted, int64_t n_sorted, int32_t sorted_dtype, int32_t side,
+                     int64_t* out, void* stream_v) {
+  SearchPlan P;
+  if (const int rc = check_search_args(src, src_dtype, sorted, n_sorted, sorted_dtype, side, &P)) return rc;
+  if (P.n == 0) return 0;
+  if (!out) return fail("bin_search: null out");
+  int sms;
+  if (const int rc = need_device(&sms)) return rc;
+  const cudaError_t e = launch_bin_search(P, sorted, (long long*)out, (cudaStream_t)stream_v);
+  if (e != cudaSuccess) return fail_cuda("bin search kernel launch", e);
   g_launches.fetch_add(1);
   return 0;
 }

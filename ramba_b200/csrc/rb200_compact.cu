@@ -43,25 +43,6 @@ template <int EB, bool FL> __device__ __forceinline__ bool c_nonzero(typename CW
   else return w != 0;
 }
 
-// element offset of C-order position p of a view
-__device__ __forceinline__ long long c_offset(const CompactView& v, long long p) {
-  if (v.nd == 1) return p * v.stride[0];
-  long long off = 0;
-#pragma unroll
-  for (int d = RB200_MAX_DIMS - 1; d >= 0; --d) {
-    if (d < v.nd) {
-      if (d == 0) {
-        off += p * v.stride[0];
-      } else {
-        const long long q = p / v.shape[d];
-        off += (p - q * v.shape[d]) * v.stride[d];
-        p = q;
-      }
-    }
-  }
-  return off;
-}
-
 // the range of positions [p0, p1) of this CTA, its first run and chunk column, and how many chunks it holds
 struct CRange {
   long long p0, p1, r0, c;

@@ -18,6 +18,27 @@ struct CompactView {
   long long stride[RB200_MAX_DIMS];  // elements
 };
 
+#ifdef __CUDACC__
+// element offset of C-order position p of a view
+__device__ __forceinline__ long long c_offset(const CompactView& v, long long p) {
+  if (v.nd == 1) return p * v.stride[0];
+  long long off = 0;
+#pragma unroll
+  for (int d = RB200_MAX_DIMS - 1; d >= 0; --d) {
+    if (d < v.nd) {
+      if (d == 0) {
+        off += p * v.stride[0];
+      } else {
+        const long long q = p / v.shape[d];
+        off += (p - q * v.shape[d]) * v.stride[d];
+        p = q;
+      }
+    }
+  }
+  return off;
+}
+#endif
+
 struct CompactPlan {
   CompactView cond;
   long long n, run_len, n_runs, cpr, runs_per_cta, ctas;

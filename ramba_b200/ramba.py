@@ -27,6 +27,7 @@ import torch
 from . import _cabi as cabi
 from . import advindex
 from . import argreduce
+from . import binning
 from . import compaction
 from . import blocks
 from . import common
@@ -2559,6 +2560,17 @@ def compress(condition, a, axis=None, out=None):
 ndarray.nonzero = nonzero
 ndarray.compress = lambda self, condition, axis=None, out=None: compress(condition, self, axis, out)
 for _n in ("nonzero", "flatnonzero", "argwhere", "count_nonzero", "extract", "compress"):
+    HANDLED_FUNCTIONS[_n] = globals()[_n]
+
+
+# ---- binning on the histogram and bin-search kernels (ramba_b200/binning.py)
+histogram = binning.histogram
+histogram_bin_edges = binning.histogram_bin_edges
+bincount = binning.bincount
+searchsorted = binning.searchsorted
+digitize = binning.digitize
+ndarray.searchsorted = lambda self, v, side="left", sorter=None: searchsorted(self, v, side, sorter)
+for _n in ("histogram", "histogram_bin_edges", "bincount", "searchsorted", "digitize"):
     HANDLED_FUNCTIONS[_n] = globals()[_n]
 
 

@@ -163,6 +163,17 @@ class CudaBackend:
         """rb200_compact on the current stream."""
         cabi.compact(cond, cond_code, run_len, counts, incl, run_base, form, values, origin, gstride, outs, self.stream_handle())
 
+    def histogram(self, view, src_code, wview, w_code, table, out, bad):
+        """rb200_histogram on the current stream; returns the scratch buffer (the caller keeps it alive)."""
+        nbytes = cabi.histogram_scratch_bytes(view, wview is not None, table)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device) if nbytes else None
+        cabi.histogram(view, src_code, wview, w_code, table, out, bad, scratch.data_ptr() if nbytes else None, self.stream_handle())
+        return scratch
+
+    def bin_search(self, view, src_code, sorted_ptr, n_sorted, sorted_code, side, out):
+        """rb200_bin_search on the current stream."""
+        cabi.bin_search(view, src_code, sorted_ptr, n_sorted, sorted_code, side, out, self.stream_handle())
+
     def init_process_group(self):
         dist.init_process_group("nccl", device_id=self.device)
 
@@ -503,6 +514,19 @@ class Runtime:
         """The payload (cabi.COMPACT_VALUES / FLAT / COORDS) of every selected element of one local condition view, in C
         order from run_base[r] + incl[q] - counts[q] for chunk q of run r (rb200_compact); outs: device addresses."""
         self.be().compact(cond, cond_code, run_len, counts, incl, run_base, form, values, origin, gstride, outs)
+        self.launches += 1
+
+    def histogram(self, view, src_code, wview, w_code, table, out, bad):
+        """This rank's B int64 counts (wview None) or float64 weight sums of one local view into out (device address),
+        binned by a cabi.BinTable (rb200_histogram); bad (device uint64) counts the elements no bin may take."""
+        keep = self.be().histogram(view, src_code, wview, w_code, table, out, bad)
+        self.launches += 1
+        return keep
+
+    def bin_search(self, view, src_code, sorted_ptr, n_sorted, sorted_code, side, out):
+        """NumPy's searchsorted of every element of one local view in a sorted device table, one int64 per element into
+        out in the view's C order (rb200_bin_search)."""
+        self.be().bin_search(view, src_code, sorted_ptr, n_sorted, sorted_code, side, out)
         self.launches += 1
 
     def gather(self, view, lin, n, out, bad):
