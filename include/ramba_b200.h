@@ -474,6 +474,79 @@ const char* rb200_describe_hist_plan(const rb200_index_view* src, int32_t weight
 int rb200_bin_search(const rb200_index_view* src, int32_t src_dtype, const void* sorted, int64_t n_sorted, int32_t sorted_dtype, int32_t side,
                      int64_t* out, void* stream);
 
+/* ---- order statistics (median, percentile, quantile) -------------------------------------------------------------------
+ * Key map.  Every element x maps to an unsigned key of KB bits (KB = 64 for F64 and I64, 32 for F32 and I32; a 32-bit
+ * key is held in the low half of a uint64) whose unsigned order is NumPy's sort order:
+ *   F64 / F32: every NaN, of any sign or payload, maps to 2^KB - 1 (after +inf); otherwise, with u the bits of x, a
+ *              clear sign bit is set (u | 2^(KB-1)) and a set sign bit flips every bit (~u).  -0.0 sorts before +0.0.
+ *   I64 / I32: the two's-complement bits with the sign bit flipped.
+ * The inverse takes a key back to the value it came from (a NaN key to the default quiet NaN).
+ * Segments.  The view's C-order positions form S = n / seg_len segments of seg_len consecutive positions (the reduced
+ * axis is the view's last dim; seg_len = n for one segment).  Each segment has K targets, each a rank in [0, seg_len):
+ * the target's key is the rank-th smallest key of its segment, counting equal keys one by one.
+ * Two forms (rb200_describe_select_plan picks one from the shapes only; RB200_NO_SELECT_ROW in the environment, read at
+ * each call, takes `row` out of the selection):
+ *   `row`  (seg_len keys fit in shared memory): rb200_select_rows.  One CTA loads its segment once, counts its NaN keys
+ *          c, and finds each target's key by 8-bit digits in shared memory; the target's rank is
+ *          rank_table[(skip_nan ? seg_len - c : 0) * K + k] (rank_table, device int64: (seg_len + 1) * K entries with
+ *          skip_nan, K otherwise).
+ *   `pass` (otherwise): the caller runs `passes` rounds of rb200_select_count then rb200_select_choose, for p = 0, 1, ...
+ *          Pass p counts the digit of `digit` bits (fewer in the last pass) below the bits chosen so far: bits
+ *          [shift_p, hi_p) with hi_p = KB - p * digit and shift_p = max(hi_p - digit, 0).  The keys of a segment that
+ *          match one of its count rows' prefixes (the chosen bits; pass 0: one row, every key) are counted per row
+ *          into counts[(s * K + row) * 2^digit + digit value] (int64, overwritten); pass 0 also writes nans[s], the NaN
+ *          keys of segment s (float sources).  With several ranks the caller sums counts (and nans) over the ranks
+ *          before the choose.  rb200_select_choose then, for each target k of each segment in order, finds the bucket
+ *          holding its residual rank in its row's counts, subtracts the keys of the lower buckets from rank[s*K+k] and
+ *          adds the bucket's bits to key[s*K+k] (pass 0 starts from 0); the targets whose keys are equal share one
+ *          count row for the next pass (n_slots[s] rows, slot[s*K+k] the target's row, slot_key its prefix), and
+ *          matched[s] is the number of keys that match a row of segment s.  After the last choose key[s*K+k] is the
+ *          target's key.  Before pass 0 the caller writes the ranks into rank[].
+ *          Candidate compaction (one segment only): mode APPEND reads the view as READ does and also appends every key
+ *          that matches a count row to cand (in no particular order: the order of keys does not change their ranks),
+ *          counting them in *cand_n (the caller zeroes it first); mode CAND reads those *cand_n keys instead of the
+ *          view.  The caller may switch to APPEND once matched[0] <= cand_cap (rb200_select_scratch_bytes / 8).
+ *          Worst case: every key in one bucket of every digit (e.g. all keys equal): no compaction, one full read of
+ *          the view per pass.                                                                                         */
+enum rb200_select_mode { RB200_SELECT_READ = 0, RB200_SELECT_APPEND = 1, RB200_SELECT_CAND = 2 };
+
+typedef struct rb200_select_state {
+  int64_t segments;      /* S                                                                                        */
+  int64_t targets;       /* K (per segment)                                                                          */
+  int64_t* rank;         /* device, S * K: the ranks before pass 0, the residual ranks after each choose             */
+  uint64_t* key;         /* device, S * K: the chosen bits; the targets' keys after the last choose                  */
+  int64_t* slot;         /* device, S * K: the target's count row                                                    */
+  uint64_t* slot_key;    /* device, S * K: each count row's prefix                                                   */
+  int64_t* n_slots;      /* device, S                                                                                */
+  int64_t* counts;       /* device, S * K * 2^digit                                                                  */
+  int64_t* nans;         /* device, S                                                                                */
+  int64_t* matched;      /* device, S                                                                                */
+  uint64_t* cand;        /* device, cand_cap keys (APPEND / CAND)                                                    */
+  int64_t cand_cap;
+  int64_t* cand_n;       /* device, 1 (APPEND / CAND)                                                                */
+  int32_t seg_dims;      /* 0: segment s of the view is row s of the state; else the view's segments, in C order over  */
+  int64_t seg_shape[RB200_MAX_DIMS];   /* seg_shape[0..seg_dims), are rows seg_base + sum(c_d * seg_gstride[d]) (a     */
+  int64_t seg_gstride[RB200_MAX_DIMS]; /* rank's block of the segments of an array cut across ranks)                  */
+  int64_t seg_base;
+} rb200_select_state;
+
+int rb200_select_count(const rb200_index_view* src, int32_t src_dtype, int64_t seg_len, const rb200_select_state* state, int32_t pass,
+                       int32_t mode, void* stream);
+int rb200_select_choose(const rb200_index_view* src, int32_t src_dtype, int64_t seg_len, const rb200_select_state* state, int32_t pass,
+                        void* stream);
+/* keys: device, S * K; nans: device, S (the NaN keys of each segment).                                                */
+int rb200_select_rows(const rb200_index_view* src, int32_t src_dtype, int64_t seg_len, int64_t targets, const int64_t* rank_table,
+                      int32_t skip_nan, uint64_t* keys, int64_t* nans, void* stream);
+/* segments = 0: the view is every segment it holds, and the form is chosen from the shapes.  segments > 0: the view holds
+ * parts of `segments` segments of an array spread over ranks; the form is `pass` and the digit width and the
+ * compaction rule follow the total.  rb200_select_count and rb200_select_choose plan with segments = state->segments.
+ * The compaction buffer's bytes (cand_cap keys of 8 bytes: max(n / 32, 65536) keys, at most n, for one segment; 0 for
+ * `row` and for several segments); -1 on a malformed argument.                                                        */
+int64_t rb200_select_scratch_bytes(const rb200_index_view* src, int32_t src_dtype, int64_t seg_len, int64_t targets, int64_t segments);
+/* One text line: form, digit width, passes, CTAs, chunk, count rows per launch (groups of them), shared bytes, count
+ * bytes and scratch bytes.  Needs no device.  NULL on a malformed argument (reason in rb200_last_error).             */
+const char* rb200_describe_select_plan(const rb200_index_view* src, int32_t src_dtype, int64_t seg_len, int64_t targets, int64_t segments);
+
 /* Which kernel rb200_run_deferred_ops would run `op` on and how (staged views, halos, TMA or cp.async loader, ring depth,
  * lean instructions, CTAs), as one text line in out[0..cap).  Needs no device and touches no pointer: the counterpart
  * of RAMBA_SHOW_CODE printing the generated kernel (ramba/ramba.py:8266-8284).                                       */

@@ -48,6 +48,8 @@ COMPACT_CHUNK = 4096
 # binning: bin-table forms (rb200_histogram) and search sides (rb200_bin_search)
 BINS_UNIFORM, BINS_EDGES, BINS_INTEGER = range(3)
 SEARCH_LEFT, SEARCH_RIGHT = range(2)
+# order statistics: count-pass modes (rb200_select_count)
+SELECT_READ, SELECT_APPEND, SELECT_CAND = range(3)
 
 
 class Insn(C.Structure):
@@ -122,6 +124,19 @@ class BinTable(C.Structure):
     ]
 
 
+class SelectState(C.Structure):
+    _fields_ = [
+        ("segments", C.c_int64), ("targets", C.c_int64),
+        ("rank", C.c_void_p), ("key", C.c_void_p), ("slot", C.c_void_p), ("slot_key", C.c_void_p), ("n_slots", C.c_void_p),
+        ("counts", C.c_void_p), ("nans", C.c_void_p), ("matched", C.c_void_p), ("cand", C.c_void_p),
+        ("cand_cap", C.c_int64),
+        ("cand_n", C.c_void_p),
+        ("seg_dims", C.c_int32),
+        ("seg_shape", C.c_int64 * MAX_DIMS), ("seg_gstride", C.c_int64 * MAX_DIMS),
+        ("seg_base", C.c_int64),
+    ]
+
+
 class RouteTable(C.Structure):
     _fields_ = [
         ("ndim", C.c_int32), ("n_ranks", C.c_int32),
@@ -176,6 +191,11 @@ EXPORTS = [
     "rb200_histogram_scratch_bytes",
     "rb200_describe_hist_plan",
     "rb200_bin_search",
+    "rb200_select_count",
+    "rb200_select_choose",
+    "rb200_select_rows",
+    "rb200_select_scratch_bytes",
+    "rb200_describe_select_plan",
 ]
 
 _LIB = None
@@ -264,6 +284,17 @@ def load():
     lib.rb200_describe_hist_plan.restype = C.c_char_p
     lib.rb200_bin_search.argtypes = [C.POINTER(IndexView), C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     lib.rb200_bin_search.restype = C.c_int
+    lib.rb200_select_count.argtypes = [C.POINTER(IndexView), C.c_int32, C.c_int64, C.POINTER(SelectState), C.c_int32, C.c_int32, C.c_void_p]
+    lib.rb200_select_count.restype = C.c_int
+    lib.rb200_select_choose.argtypes = [C.POINTER(IndexView), C.c_int32, C.c_int64, C.POINTER(SelectState), C.c_int32, C.c_void_p]
+    lib.rb200_select_choose.restype = C.c_int
+    lib.rb200_select_rows.argtypes = [C.POINTER(IndexView), C.c_int32, C.c_int64, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                      C.c_void_p]
+    lib.rb200_select_rows.restype = C.c_int
+    lib.rb200_select_scratch_bytes.argtypes = [C.POINTER(IndexView), C.c_int32, C.c_int64, C.c_int64, C.c_int64]
+    lib.rb200_select_scratch_bytes.restype = C.c_int64
+    lib.rb200_describe_select_plan.argtypes = [C.POINTER(IndexView), C.c_int32, C.c_int64, C.c_int64, C.c_int64]
+    lib.rb200_describe_select_plan.restype = C.c_char_p
     if lib.rb200_abi_version() != ABI_VERSION:
         raise CabiError("libramba_b200.so ABI %d != binding ABI %d: rebuild" % (lib.rb200_abi_version(), ABI_VERSION))
     _LIB = lib
@@ -488,3 +519,35 @@ def describe_hist_plan(src, weighted, table):
 def bin_search(src, src_dtype, sorted_ptr, n_sorted, sorted_dtype, side, out, stream=None):
     """rb200_bin_search: out[p] (device int64, the view's C order) = NumPy's searchsorted of every element."""
     check(load().rb200_bin_search(C.byref(src), src_dtype, _p(sorted_ptr), n_sorted, sorted_dtype, side, _p(out), _p(stream)))
+
+
+def select_count(src, src_dtype, seg_len, state, pass_, mode, stream=None):
+    """rb200_select_count: one count pass of the `pass` form over this view (or the candidate keys) into state.counts."""
+    check(load().rb200_select_count(C.byref(src), src_dtype, seg_len, C.byref(state), pass_, mode, _p(stream)))
+
+
+def select_choose(src, src_dtype, seg_len, state, pass_, stream=None):
+    """rb200_select_choose: every target's bucket of pass pass_, on the device."""
+    check(load().rb200_select_choose(C.byref(src), src_dtype, seg_len, C.byref(state), pass_, _p(stream)))
+
+
+def select_rows(src, src_dtype, seg_len, targets, rank_table, skip_nan, keys, nans, stream=None):
+    """rb200_select_rows: the `row` form, every target's key of every segment in one launch."""
+    check(load().rb200_select_rows(C.byref(src), src_dtype, seg_len, targets, _p(rank_table), int(bool(skip_nan)), _p(keys), _p(nans),
+                                   _p(stream)))
+
+
+def select_scratch_bytes(src, src_dtype, seg_len, targets, segments=0):
+    n = load().rb200_select_scratch_bytes(C.byref(src), src_dtype, seg_len, targets, segments)
+    if n < 0:
+        check(1)
+    return n
+
+
+def describe_select_plan(src, src_dtype, seg_len, targets, segments=0):
+    """One text line: the form, digit width, passes, CTAs and buffer sizes the library would select with (no device);
+    segments > 0: the view is a rank's part of that many segments (the pass form)."""
+    s = load().rb200_describe_select_plan(C.byref(src), src_dtype, seg_len, targets, segments)
+    if s is None:
+        check(1)
+    return s.decode()

@@ -12,6 +12,7 @@
 #include "rb200_argred.h"
 #include "rb200_compact.h"
 #include "rb200_hist.h"
+#include "rb200_select.h"
 #include "rb200_group.h"
 #include "rb200_index.h"
 #include "rb200_rng.h"
@@ -473,6 +474,35 @@ static int check_search_args(const rb200_index_view* src, int src_dtype, const v
   return 0;
 }
 
+// ---- order statistics: argument checks (before any device query) and the plan
+static int check_select_plan(const rb200_index_view* src, int src_dtype, long long seg_len, long long targets, long long segments, SelectPlan* P) {
+  if (const int rc = check_index_view(src, "select")) return rc;
+  if (!bins_src_dtype(src_dtype)) return fail("select: source dtype must be float64/float32/int64/int32");
+  if (dtype_size(src_dtype) != src->elem_bytes) return fail("select: elem_bytes does not match the source dtype");
+  long long n = 1;
+  for (int d = 0; d < src->ndim; ++d) n *= src->shape[d];
+  if (seg_len < 1) return fail("select: seg_len must be at least 1");
+  if (n % seg_len != 0) return fail("select: seg_len does not divide the view's size");
+  if (targets < 1 || targets > (1ll << 20)) return fail("select: targets must be in 1 .. 2^20");
+  if (segments < 0) return fail("select: negative segments");
+  if (segments > 0 && n / seg_len > segments) return fail("select: the view holds more segments than the array");
+  make_select_plan(*src, src_dtype, seg_len, targets, segments, getenv("RB200_NO_SELECT_ROW") != nullptr, P);
+  return 0;
+}
+
+static int check_select_state(const SelectPlan& P, const rb200_select_state* st, int pass, const char* who) {
+  const std::string w(who);
+  if (!st) return fail(w + ": null state");
+  if (st->seg_dims < 0 || st->seg_dims > RB200_MAX_DIMS) return fail(w + ": seg_dims out of range");
+  if (st->seg_dims == 0 && st->segments != P.S && P.n > 0) return fail(w + ": state segments differ from the view's");
+  if (pass < 0 || pass >= P.passes) return fail(w + ": pass out of range");
+  if (P.GS > 0 && (!st->rank || !st->key || !st->slot || !st->slot_key || !st->n_slots || !st->counts || !st->nans || !st->matched))
+    return fail(w + ": null state buffer");
+  return 0;
+}
+
+static thread_local std::string g_select_plan_text;
+
 extern "C" {
 
 const char* rb200_last_error(void) { return g_last_error.c_str(); }
@@ -767,6 +797,75 @@ int rb200_bin_search(const rb200_index_view* src, int32_t src_dtype, const void*
   if (const int rc = need_device(&sms)) return rc;
   const cudaError_t e = launch_bin_search(P, sorted, (long long*)out, (cudaStream_t)stream_v);
   if (e != cudaSuccess) return fail_cuda("bin search kernel launch", e);
+  g_launches.fetch_add(1);
+  return 0;
+}
+
+const char* rb200_describe_select_plan(const rb200_index_view* src, int32_t src_dtype, int64_t seg_len, int64_t targets, int64_t segments) {
+  SelectPlan P;
+  if (check_select_plan(src, src_dtype, seg_len, targets, segments, &P)) return nullptr;
+  char buf[320];
+  snprintf(buf, sizeof(buf),
+           "kernel=select form=%s segments=%lld all_segments=%lld seg_len=%lld targets=%lld digit=%d passes=%d ctas=%lld chunk=%lld rows=%lld groups=%lld "
+           "shared_bytes=%lld counts_bytes=%lld scratch_bytes=%lld load=%s",
+           select_form_name(P.form), P.S, P.GS, P.L, P.K, P.digit, P.passes, P.ctas, P.chunk, P.rows, P.groups, P.shared_bytes, P.counts_bytes,
+           P.cand_cap * 8, P.vec ? "vector" : "strided");
+  g_select_plan_text = buf;
+  return g_select_plan_text.c_str();
+}
+
+int64_t rb200_select_scratch_bytes(const rb200_index_view* src, int32_t src_dtype, int64_t seg_len, int64_t targets, int64_t segments) {
+  SelectPlan P;
+  if (check_select_plan(src, src_dtype, seg_len, targets, segments, &P)) return -1;
+  return P.cand_cap * 8;
+}
+
+int rb200_select_count(const rb200_index_view* src, int32_t src_dtype, int64_t seg_len, const rb200_select_state* state, int32_t pass,
+                       int32_t mode, void* stream_v) {
+  SelectPlan P;
+  if (!state) return fail("select_count: null state");
+  if (const int rc = check_select_plan(src, src_dtype, seg_len, state->targets, std::max<long long>(state->segments, 1), &P)) return rc;
+  if (const int rc = check_select_state(P, state, pass, "select_count")) return rc;
+  if (mode != RB200_SELECT_READ && mode != RB200_SELECT_APPEND && mode != RB200_SELECT_CAND) return fail("select_count: bad mode");
+  if (mode != RB200_SELECT_READ) {
+    if (P.GS != 1) return fail("select_count: candidate compaction needs one segment");
+    if (pass == 0) return fail("select_count: candidate compaction needs a chosen prefix (pass >= 1)");
+    if (!state->cand || !state->cand_n || state->cand_cap < 1)
+      return fail("select_count: bad candidate buffer");
+  }
+  int sms;
+  if (const int rc = need_device(&sms)) return rc;
+  const cudaError_t e = launch_select_count(P, *state, pass, mode, (cudaStream_t)stream_v);
+  if (e != cudaSuccess) return fail_cuda("select count kernel launch", e);
+  g_launches.fetch_add(1);
+  return 0;
+}
+
+int rb200_select_choose(const rb200_index_view* src, int32_t src_dtype, int64_t seg_len, const rb200_select_state* state, int32_t pass,
+                        void* stream_v) {
+  SelectPlan P;
+  if (!state) return fail("select_choose: null state");
+  if (const int rc = check_select_plan(src, src_dtype, seg_len, state->targets, std::max<long long>(state->segments, 1), &P)) return rc;
+  if (const int rc = check_select_state(P, state, pass, "select_choose")) return rc;
+  int sms;
+  if (const int rc = need_device(&sms)) return rc;
+  const cudaError_t e = launch_select_choose(P, *state, pass, (cudaStream_t)stream_v);
+  if (e != cudaSuccess) return fail_cuda("select choose kernel launch", e);
+  g_launches.fetch_add(1);
+  return 0;
+}
+
+int rb200_select_rows(const rb200_index_view* src, int32_t src_dtype, int64_t seg_len, int64_t targets, const int64_t* rank_table,
+                      int32_t skip_nan, uint64_t* keys, int64_t* nans, void* stream_v) {
+  SelectPlan P;
+  if (const int rc = check_select_plan(src, src_dtype, seg_len, targets, 0, &P)) return rc;
+  if (P.form != SELECT_ROW) return fail("select_rows: the segments do not fit in shared memory (rb200_select_count)");
+  if (P.S > 0 && (!rank_table || !keys || !nans)) return fail("select_rows: null rank table, keys or nans");
+  int sms;
+  if (const int rc = need_device(&sms)) return rc;
+  const cudaError_t e = launch_select_rows(P, (const long long*)rank_table, skip_nan != 0, (unsigned long long*)keys, (long long*)nans,
+                                           (cudaStream_t)stream_v);
+  if (e != cudaSuccess) return fail_cuda("select row kernel launch", e);
   g_launches.fetch_add(1);
   return 0;
 }

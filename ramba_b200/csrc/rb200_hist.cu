@@ -232,11 +232,8 @@ __global__ void __launch_bounds__(kHThreads, 2) hist_kernel(const __grid_constan
           }
           __syncwarp();
         } else {
-          // counts: a warp whose lanes all fall into one bin adds 32 once; otherwise every lane adds its own element
-          const unsigned k0 = __shfl_sync(0xffffffffu, key, 0);
-          const bool one = __all_sync(0xffffffffu, key == k0);
-          const unsigned add = one ? 32u : 1u;
-          if (key != 0xffffffffu && (!one || lane == 0)) {
+          const unsigned add = warp_bin_share(key, lane);
+          if (add) {
             if constexpr (GLOBAL) atomicAdd(reinterpret_cast<unsigned long long*>(A.out) + bin, (unsigned long long)add);
             else atomicAdd(rows_u + key, add);
           }
@@ -347,15 +344,9 @@ void make_search_plan(const rb200_index_view& src, long long n_tab, int tab_dtyp
   p.shared_bytes = p.table_shared ? tb : 0;
 }
 
-// kernels that stage more than 48 KB must ask for it
-template <class K> static cudaError_t h_allow_shared(K kernel, long long smem) {
-  if (smem <= 48 * 1024) return cudaSuccess;
-  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-}
-
 template <class T, bool W, bool GLOBAL> static cudaError_t hist_t(const HistArgs& A, cudaStream_t s) {
   const auto k = hist_kernel<T, W, GLOBAL>;
-  if (const cudaError_t e = h_allow_shared(k, A.P.shared_bytes)) return e;
+  if (const cudaError_t e = allow_shared(k, A.P.shared_bytes)) return e;
   k<<<(unsigned)A.P.ctas, kHThreads, (size_t)A.P.shared_bytes, s>>>(A);
   return cudaGetLastError();
 }
@@ -401,7 +392,7 @@ cudaError_t launch_histogram(const HistPlan& P, const rb200_bin_table& T, const 
 
 template <class T, class C> static cudaError_t search_t(const SearchArgs& A, cudaStream_t s) {
   const auto k = search_kernel<T, C>;
-  if (const cudaError_t e = h_allow_shared(k, A.P.shared_bytes)) return e;
+  if (const cudaError_t e = allow_shared(k, A.P.shared_bytes)) return e;
   k<<<(unsigned)A.P.ctas, kSThreads, (size_t)A.P.shared_bytes, s>>>(A);
   return cudaGetLastError();
 }

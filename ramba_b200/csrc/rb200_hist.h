@@ -39,4 +39,22 @@ cudaError_t launch_histogram(const HistPlan& P, const rb200_bin_table& T, const 
 cudaError_t launch_bin_search(const SearchPlan& P, const void* table, long long* out, cudaStream_t stream);
 const char* hist_form_name(int form);
 
+// kernels that stage more than 48 KB of dynamic shared memory must ask for it
+template <class K> static inline cudaError_t allow_shared(K kernel, long long smem) {
+  if (smem <= 48 * 1024) return cudaSuccess;
+  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+}
+
+#ifdef __CUDACC__
+// What this lane adds to privatised bin `key` (0xffffffff: no bin) so that the warp adds one per lane that has a bin:
+// a warp whose 32 lanes fall into one bin adds 32 once from lane 0 (data skewed into one bin), otherwise every lane
+// adds 1.  Every lane of the warp calls it.
+__device__ __forceinline__ unsigned warp_bin_share(unsigned key, int lane) {
+  const unsigned k0 = __shfl_sync(0xffffffffu, key, 0);
+  const bool one = __all_sync(0xffffffffu, key == k0);
+  if (key == 0xffffffffu) return 0u;
+  return one ? (lane == 0 ? 32u : 0u) : 1u;
+}
+#endif
+
 }  // namespace rb200

@@ -28,6 +28,7 @@ from . import _cabi as cabi
 from . import advindex
 from . import argreduce
 from . import binning
+from . import quantile as _quantile_mod
 from . import compaction
 from . import blocks
 from . import common
@@ -2571,6 +2572,17 @@ searchsorted = binning.searchsorted
 digitize = binning.digitize
 ndarray.searchsorted = lambda self, v, side="left", sorter=None: searchsorted(self, v, side, sorter)
 for _n in ("histogram", "histogram_bin_edges", "bincount", "searchsorted", "digitize"):
+    HANDLED_FUNCTIONS[_n] = globals()[_n]
+
+
+# ---- order statistics on the radix-select kernels (ramba_b200/quantile.py)
+median = _quantile_mod.median
+nanmedian = _quantile_mod.nanmedian
+percentile = _quantile_mod.percentile
+nanpercentile = _quantile_mod.nanpercentile
+quantile = _quantile_mod.quantile
+nanquantile = _quantile_mod.nanquantile
+for _n in ("median", "nanmedian", "percentile", "nanpercentile", "quantile", "nanquantile"):
     HANDLED_FUNCTIONS[_n] = globals()[_n]
 
 

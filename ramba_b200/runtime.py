@@ -174,6 +174,18 @@ class CudaBackend:
         """rb200_bin_search on the current stream."""
         cabi.bin_search(view, src_code, sorted_ptr, n_sorted, sorted_code, side, out, self.stream_handle())
 
+    def select_count(self, view, src_code, seg_len, state, pass_, mode):
+        """rb200_select_count on the current stream."""
+        cabi.select_count(view, src_code, seg_len, state, pass_, mode, self.stream_handle())
+
+    def select_choose(self, view, src_code, seg_len, state, pass_):
+        """rb200_select_choose on the current stream."""
+        cabi.select_choose(view, src_code, seg_len, state, pass_, self.stream_handle())
+
+    def select_rows(self, view, src_code, seg_len, targets, rank_table, skip_nan, keys, nans):
+        """rb200_select_rows on the current stream."""
+        cabi.select_rows(view, src_code, seg_len, targets, rank_table, skip_nan, keys, nans, self.stream_handle())
+
     def init_process_group(self):
         dist.init_process_group("nccl", device_id=self.device)
 
@@ -527,6 +539,23 @@ class Runtime:
         """NumPy's searchsorted of every element of one local view in a sorted device table, one int64 per element into
         out in the view's C order (rb200_bin_search)."""
         self.be().bin_search(view, src_code, sorted_ptr, n_sorted, sorted_code, side, out)
+        self.launches += 1
+
+    def select_count(self, view, src_code, seg_len, state, pass_, mode):
+        """One count pass of the radix select over one local view (or the candidate keys of mode SELECT_CAND) into the
+        device counts of a cabi.SelectState (rb200_select_count)."""
+        self.be().select_count(view, src_code, seg_len, state, pass_, mode)
+        self.launches += 1
+
+    def select_choose(self, view, src_code, seg_len, state, pass_):
+        """Every target's bucket of one pass, from the (summed) counts, on the device (rb200_select_choose)."""
+        self.be().select_choose(view, src_code, seg_len, state, pass_)
+        self.launches += 1
+
+    def select_rows(self, view, src_code, seg_len, targets, rank_table, skip_nan, keys, nans):
+        """Every target's key of every segment of one local view, one CTA per segment in shared memory
+        (rb200_select_rows)."""
+        self.be().select_rows(view, src_code, seg_len, targets, rank_table, skip_nan, keys, nans)
         self.launches += 1
 
     def gather(self, view, lin, n, out, bad):
