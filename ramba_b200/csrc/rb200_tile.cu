@@ -597,8 +597,11 @@ bool plan_stencil_tile(const rb200_fused_op* op, int sms, bool use_terms, bool u
   };
   tb.ctx = &P;
   P.elem = es;
-  if (!use_terms || !build_terms(tb, P.insns, P.n_insns, P.terms, kTileMaxTerms, &P.n_terms, &P.n32, &P.out_view)) {
+  // the term kernel runs a float32 phase only on float32 staged data (stencil_terms_kernel<float, 8>); a float64 group
+  // behind a float32 prefix takes the lean machine, which runs every class
+  if (!use_terms || !build_terms(tb, P.insns, P.n_insns, P.terms, kTileMaxTerms, &P.n_terms, &P.n32, &P.out_view) || (es == 8 && P.n32 > 0)) {
     P.n_terms = 0;
+    P.n32 = 0;
     int n_chain = 0;
     P.n_insns = lean_fuse_chains(P.insns, P.n_insns, P.chain, kTileMaxChain, &n_chain);
   } else {
@@ -658,8 +661,11 @@ bool plan_stencil_tile(const rb200_fused_op* op, int sms, bool use_terms, bool u
   T.smem = smem;
   T.es = es;
   T.nd = nd;
-  // ---- can the halo'd source box be described by a TMA tensor map?  (strides multiples of 16 bytes, base moved down
-  // to 16-byte alignment, the whole box inside the shard buffer)
+  // ---- can the halo'd source box be described by a TMA tensor map?  (strides multiples of 16 bytes, the corner on a
+  // 16-byte boundary, rows of whole 16-byte units, the whole box inside the shard buffer.)  On an H100, bulk tensor copies
+  // from maps whose base had been moved down to the boundary (shift > 0) stopped the kernel with an illegal instruction;
+  // those maps' rows also ended inside a 16-byte unit and the cause is not known, so as a precaution TMA is taken only
+  // where both conditions hold (DESIGN §3.4).  The shift stays in the map and kernel parameters, always 0 here.
   if (P.has_group) {
     const uintptr_t corner = (uintptr_t)P.gcorner;
     T.shift = (int)((corner & 15u) / (unsigned)es);
@@ -672,7 +678,7 @@ bool plan_stencil_tile(const rb200_fused_op* op, int sms, bool use_terms, bool u
     const char* ahi = (const char*)op->views[best_ref].alloc_hi;
     const bool aligned = (P.gs1 * es) % 16 == 0 && (nd == 2 || ((P.gs0 * es) % 16 == 0 && P.gs0 > 0)) && (corner % (unsigned)es) == 0;
     const bool inside = T.tbase >= alo && far_end <= ahi;
-    T.tma_ok = use_tma && aligned && inside && T.Xh < (1ll << 31);
+    T.tma_ok = use_tma && aligned && inside && T.shift == 0 && (T.Xh * es) % 16 == 0 && T.Xh < (1ll << 31);
   }
   return true;
 }
@@ -688,9 +694,10 @@ std::string describe_stencil_tile(const TilePlan& T) {
   char buf[400];
   snprintf(buf, sizeof(buf),
            "kernel=%s elem=%d box=%lldx%lldx%lld staged_views=%d halo=z%d+%d,y%d+%d,x%d+%d ring=%d loader=%s direct_views=%d lean_insns=%d "
-           "chains=%d chain_steps=%d terms=%d(f32:%d) tile=128x%d items=%lld planes_per_item=%lld ctas=%lld smem=%zu",
+           "chains=%d chain_steps=%d terms=%d(f32:%d) fast_tail=%d tile=128x%d items=%lld planes_per_item=%lld ctas=%lld smem=%zu corner_shift=%d",
            P.n_terms > 0 ? "stencil_terms" : "stencil_tile", T.es, P.Z, P.Y, P.X, P.n_staged, P.hz_lo, P.hz - P.hz_lo, P.hy_lo, P.hy - P.hy_lo, P.hx_lo, P.hx - P.hx_lo, P.D,
-           !P.has_group ? "none" : (T.tma_ok ? "tma" : "cp.async"), P.n_direct, P.n_insns, n_chain_insns, n_chain_steps, P.n_terms, P.n32, P.tv * kTileRY, P.n_items, P.ZC, T.blocks, T.smem);
+           !P.has_group ? "none" : (T.tma_ok ? "tma" : "cp.async"), P.n_direct, P.n_insns, n_chain_insns, n_chain_steps, P.n_terms, P.n32, P.fast_tail, P.tv * kTileRY, P.n_items,
+           P.ZC, T.blocks, T.smem, P.has_group ? T.shift : 0);
   return buf;
 }
 

@@ -39,7 +39,7 @@ struct TileParams {
   long long gs0, gs1;                    // group strides (elements) of z and y; x stride is 1
   const char* safe_lo;                   // [safe_lo, safe_hi): bytes the cooperative loader may touch
   const char* safe_hi;
-  int tma_shift;                         // elements the tensor-map base was moved down to reach 16-byte alignment
+  int tma_shift;                         // elements the tensor-map base was moved down (0: the planner takes TMA only for aligned corners)
   int n_staged;
   TileStagedOp staged[kTileMaxStaged];
   int n_direct;

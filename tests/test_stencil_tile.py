@@ -2,13 +2,21 @@
 the oracle executor (CPU, always) and through the CUDA library (-m gpu), BIT-exact on arbitrary float data (both
 sides do the same operations in the same order and classes, one rounding each).  Shapes cover the TMA path (row
 strides that are multiples of 16 bytes), the cooperative cp.async path (odd row lengths, unaligned corners), ragged
-tiles, 2-D and 3-D, float32 and float64, wide halos, several source arrays, in-place accumulation."""
+tiles, 2-D and 3-D, float32 and float64, wide halos, several source arrays, in-place accumulation.
+
+With np = NumPy each program computes its expected value with the engine's per-operation classes written out (Numba's
+typing: float32 op float32 rounds in float32, float32 op a Python float is a float64 operation, the store converts), so
+the oracle leg compares bit for bit too."""
 import numpy as onp
 import pytest
 
 
 def _h(x):
     return x.asarray() if hasattr(x, "asarray") else onp.asarray(x)
+
+
+def _f64(x):
+    return onp.asarray(x).astype(onp.float64)
 
 
 def _data(shape, dtype, seed):
@@ -21,6 +29,10 @@ def lap3d(np, n0, n1, n2, dtype, seed=0):
     Uh = _data((n0, n1, n2), dtype, seed)
     U = Uh if np is onp else np.fromarray(Uh)
     V = np.zeros((n0, n1, n2), dtype=dtype)
+    if np is onp:
+        s = U[:-2, 1:-1, 1:-1] + U[2:, 1:-1, 1:-1] + U[1:-1, :-2, 1:-1] + U[1:-1, 2:, 1:-1] + U[1:-1, 1:-1, :-2] + U[1:-1, 1:-1, 2:]
+        V[1:-1, 1:-1, 1:-1] = _f64(s) - 6.0 * _f64(U[1:-1, 1:-1, 1:-1])
+        return [V]
     V[1:-1, 1:-1, 1:-1] = (U[:-2, 1:-1, 1:-1] + U[2:, 1:-1, 1:-1] + U[1:-1, :-2, 1:-1] + U[1:-1, 2:, 1:-1]
                            + U[1:-1, 1:-1, :-2] + U[1:-1, 1:-1, 2:] - 6.0 * U[1:-1, 1:-1, 1:-1])
     return [_h(V)]
@@ -29,14 +41,20 @@ def lap3d(np, n0, n1, n2, dtype, seed=0):
 def star2d(np, n, m, dtype, r, seed=1):
     """PRK-style star stencil of radius r with weights, accumulated into the output (README.md:271-299)."""
     Ah = _data((n, m), dtype, seed)
-    A = Ah if np is onp else np.fromarray(Ah)
+    A = _f64(Ah) if np is onp else np.fromarray(Ah)  # (every weighted term is a float64 operation)
     B = np.ones((n, m), dtype=dtype)
     acc = None
     for j in range(1, r + 1):
         w = 1.0 / (2.0 * j * r)
         t = (w * A[r:-r, r + j:m - r + j] - w * A[r:-r, r - j:m - r - j]
              + w * A[r + j:n - r + j, r:-r] - w * A[r - j:n - r - j, r:-r])
+        if np is onp and j == r:
+            # the last t is still named by a Python variable when B is updated, so the engine stores it (rounded to the
+            # data's dtype); earlier t's and partial sums are never stored and keep their float64 values
+            t = _f64(t.astype(dtype))
         acc = t if acc is None else acc + t
+    if np is onp:
+        acc = acc.astype(dtype)  # (acc is stored too)
     B[r:-r, r:-r] += acc
     return [_h(B)]
 
@@ -51,7 +69,7 @@ def box2d(np, n, m, dtype, seed=2):
         for dx in (0, 1, 2):
             v = A[dy:n - 2 + dy, dx:m - 2 + dx]
             s = v if s is None else s + v
-    out[1:-1, 1:-1] = s * W[1:-1, 1:-1] * 0.125
+    out[1:-1, 1:-1] = _f64(s * W[1:-1, 1:-1]) * 0.125 if np is onp else s * W[1:-1, 1:-1] * 0.125
     return [_h(out)]
 
 
@@ -60,6 +78,9 @@ def asym3d(np, n0, n1, n2, dtype, seed=3):
     Uh = _data((n0, n1, n2), dtype, seed)
     U = Uh if np is onp else np.fromarray(Uh)
     V = np.zeros((n0 - 2, n1 - 1, n2 - 3), dtype=dtype)
+    if np is onp:
+        V[:, :, :] = _f64(U[2:, 1:, 3:]) - 0.5 * _f64(U[1:-1, 1:, 3:]) - 0.25 * _f64(U[:-2, 1:, 3:]) + _f64(U[2:, :-1, 3:] * U[2:, 1:, :-3])
+        return [V]
     V[:, :, :] = U[2:, 1:, 3:] - 0.5 * U[1:-1, 1:, 3:] - 0.25 * U[:-2, 1:, 3:] + U[2:, :-1, 3:] * U[2:, 1:, :-3]
     return [_h(V)]
 
@@ -70,6 +91,10 @@ def elementwise_nd(np, shape, dtype, seed=4):
     A, B = (Ah, Bh) if np is onp else (np.fromarray(Ah), np.fromarray(Bh))
     row = A[0] * 2.0
     sl = tuple(slice(1, None, 2) for _ in shape)
+    if np is onp:
+        dt = Ah.dtype
+        return [(_f64(A[sl] * B[sl]) - 0.5 * _f64(A[sl])).astype(dt), (_f64(A + row) * 0.5).astype(dt),
+                (abs(_f64(A.T) - 1.0) + _f64(B.T * B.T)).astype(dt), (_f64(onp.minimum(A[sl], B[sl])) - onp.maximum(_f64(A[sl]), 0.25)).astype(dt)]
     return [_h(A[sl] * B[sl] - 0.5 * A[sl]), _h((A + row) * 0.5), _h(abs(A.T - 1.0) + B.T * B.T), _h(np.minimum(A[sl], B[sl]) - np.maximum(A[sl], 0.25))]
 
 
@@ -103,15 +128,11 @@ def _exact(got, exp, name):
 
 @pytest.mark.parametrize("name,prog", CASES, ids=[c[0] for c in CASES])
 def test_stencil_oracle_vs_numpy(oracle_engine, name, prog):
-    """Host logic + oracle: the op list the fuser builds means what NumPy computes (float64 data: NumPy evaluates the
-    same operations in the same order; float32 data with Python-float weights is computed in float64 by the op list, as
-    Numba does in the reference, so those cases are compared with a tolerance here and bit-exactly on the GPU leg)."""
+    """Host logic + oracle: the op list the fuser builds means what the program's NumPy restatement computes with the
+    engine's per-operation classes, bit for bit."""
     import ramba_b200 as rb
 
-    got, exp = prog(rb), prog(onp)
-    for g, e in zip(got, exp):
-        assert g.shape == e.shape and g.dtype == e.dtype
-        assert onp.allclose(g, e, rtol=1e-5 if e.dtype == onp.float32 else 1e-12, atol=1e-5 if e.dtype == onp.float32 else 1e-12), name
+    _exact(prog(rb), prog(onp), name)
 
 
 @pytest.mark.gpu
